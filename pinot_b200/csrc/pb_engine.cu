@@ -100,12 +100,8 @@ static int init_context(Context* c) {
     cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
   }
   // the aggregation kernel gathers 4-8 bytes at random docIds: fetch single 32-byte sectors from DRAM instead of
-  // the default 64 (PB_L2_FETCH=64|128 restores the larger granularity for A/B measurements)
-  {
-    size_t gran = 32;
-    if (const char* e = getenv("PB_L2_FETCH")) gran = (size_t)atoi(e);
-    if (gran == 32 || gran == 64 || gran == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, gran);
-  }
+  // the default 64
+  cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
   CU(cudaStreamCreateWithFlags(&c->util_stream, cudaStreamNonBlocking));
   CU(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
   return PB_OK;
@@ -1005,6 +1001,9 @@ struct TableMeta {
   uint64_t out_cap = 0;                     // capacity of the pinned output arrays
 };
 
+// The aggregation kernel of a plan (AGG_NONE: the call has no docs, nothing to aggregate)
+enum AggKernel { AGG_NONE, AGG_GENERAL, AGG_SMEM, AGG_ROWS };   // pb_agg_kernel<6>, pb_agg_smem_kernel, pb_agg_rows_kernel
+
 struct pb_result_s {
   pb_group_s* group = nullptr;
   cudaStream_t stream = nullptr;
@@ -1015,7 +1014,6 @@ struct pb_result_s {
   int n_agg_filters = 0;
   bool count_all = false;                   // PB_Q_NULL_HANDLING: every aggregation keeps its own (non-null) row count
   std::vector<int> agg_filter_of;
-  int waves = 1;                            // launches were split into this many waves behind the staging copies
   int in_place_columns = 0;                 // (segment, column) pairs gathered from mapped host memory (PB_Q_GATHER_IN_PLACE)
   std::vector<int> agg_op;
   std::vector<std::string> gb_names, agg_cols;
@@ -1024,15 +1022,12 @@ struct pb_result_s {
   void* scratch = nullptr; size_t scratch_cap = 0;   // cached large scratch (match list)
   unsigned long long* d_counters = nullptr; // per table: [num_groups(u32 pair), limit flag, docs_matched, compaction counter]
   HostArr h_counters;
-  int n_distinct_cols = 0;
-  int n_scan_leaves_total = 0;
   std::vector<int64_t> seg_scan_leaves;     // per segment: number of scan leaves (for numEntriesScannedInFilter)
   double device_ms = 0, scan_ms = 0;
   double host_us[8] = {0};   // [0] stage+resolve [1] tables [2] descriptors [3] launches [4] finalize: count [5] gather+D2H wait [6] host decode
   int launches = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, ev2 = nullptr, ev3 = nullptr;
   StreamSet sset;
-  bool match_all = false;
   double filter_ms = 0, agg_ms = 0;
   // contiguous spans of table 0 for the cross-GPU reduce: [counters .. row counts] int64 SUM, sums float64 SUM, min/max int64 MIN
   unsigned long long* span_i64 = nullptr; int64_t span_i64_n = 0;
@@ -1051,8 +1046,8 @@ struct pb_result_s {
     const DevExpandItem* expand_items = nullptr; int n_expand = 0;
     int U = 2; bool u2_three = false; size_t smem_filter = 0;
     int spec_w = 0, spec_pk = 0;             // > 0: the plan-time specialised filter kernel of that width / predicate kind
-    const DevRowSeg* row_segs = nullptr; int rows_rw = 0;   // agg_kind 4: pb_agg_rows_kernel<rows_rw>
-    int agg_kind = 0;                        // 0 none (fused), 1 pb_agg_kernel<6>, 2 pb_agg_kernel<4>, 3 pb_agg_smem_kernel
+    const DevRowSeg* row_segs = nullptr; int rows_rw = 0;   // AGG_ROWS: pb_agg_rows_kernel<rows_rw>
+    AggKernel agg = AGG_NONE;
     size_t smem_agg = 0;
     const DevLaneWeights* lane_w = nullptr; int n_lanes = 0, n_segs = 0;
     std::vector<DevFinalize> fin; std::vector<int> fin_grid; bool fin_prepared = false;
@@ -1065,7 +1060,6 @@ struct pb_result_s {
     cudaGraphExec_t graph = nullptr;
     int uses = 0, graph_launches = 0;
     double comm_ms_sample = 0;               // cross-rank merge time of the plan's last kernel-by-kernel run (graph replays repeat it)
-    uint32_t flags = 0;
   } rp;
   bool graph_replayed = false;
   struct InitArgs { uint4* zero = nullptr; uint64_t zn = 0; uint4* ff = nullptr; uint64_t fn = 0; uint4* mm = nullptr; uint64_t mn = 0;
@@ -1076,7 +1070,6 @@ struct pb_result_s {
   std::vector<unsigned long long*> d_okey; std::vector<DevSelectState*> d_sel;
   bool track_first = false; uint32_t* d_first_thr = nullptr;   // numGroupsLimit in doc order (dense per-segment tables)
   bool repair_pass = false;                 // hash tables with a reachable numGroupsLimit: conditional second aggregation pass
-  bool fused = false, smem_table = false;   // how the matches reached the table (see exec_single)
   bool comm_timed = false;                  // events [5],[6] bracket the cross-rank merge
   double comm_ms = 0;
   Context* ctx = nullptr;
@@ -1532,7 +1525,7 @@ static int enqueue_all(pb_result_s* r, const std::vector<cudaEvent_t>* seg_wait)
     r->launches++;
   }
   CU(cudaGetLastError());
-  // kernel 1: filter -> match list (or fused aggregation);  kernel 2: gather + aggregate the matching docs (per wave)
+  // kernel 1: filter -> match list;  kernel 2: gather + aggregate the matching docs (per wave)
   CU(cudaEventRecord(r->ev1, st));
   for (size_t wi = 0; wi < rp.waves.size(); wi++) {
     const pb_result_s::WaveLaunch& w = rp.waves[wi];
@@ -1550,16 +1543,15 @@ static int enqueue_all(pb_result_s* r, const std::vector<cudaEvent_t>* seg_wait)
     }
     if (wi + 1 == rp.waves.size() || rp.waves.size() == 1) CU(cudaEventRecord(r->evm, st));   // (waves interleave: the split is only exact for one wave)
     if (w.grid_agg > 0) {
-      if (rp.agg_kind == 4) {
+      if (rp.agg == AGG_ROWS) {
         if (rp.rows_rw == 2) pb_agg_rows_kernel<2><<<w.grid_agg, PB_AGG_SMEM_THREADS, rp.smem_agg, st>>>(w.dq, rp.row_segs);
         else if (rp.rows_rw == 4) pb_agg_rows_kernel<4><<<w.grid_agg, PB_AGG_SMEM_THREADS, rp.smem_agg, st>>>(w.dq, rp.row_segs);
         else pb_agg_rows_kernel<8><<<w.grid_agg, PB_AGG_SMEM_THREADS, rp.smem_agg, st>>>(w.dq, rp.row_segs);
-      } else if (rp.agg_kind == 3) pb_agg_smem_kernel<<<w.grid_agg, PB_AGG_SMEM_THREADS, rp.smem_agg, st>>>(w.dq);
-      else if (rp.agg_kind == 2) pb_agg_kernel<4><<<w.grid_agg, PB_NTHREADS, rp.smem_agg, st>>>(w.dq);
+      } else if (rp.agg == AGG_SMEM) pb_agg_smem_kernel<<<w.grid_agg, PB_AGG_SMEM_THREADS, rp.smem_agg, st>>>(w.dq);
       else pb_agg_kernel<6><<<w.grid_agg, PB_NTHREADS, rp.smem_agg, st>>>(w.dq);
       r->launches++;
       CU(cudaGetLastError());
-      if (r->repair_pass && rp.waves.size() == 1 && (rp.agg_kind == 1 || rp.agg_kind == 2)) {
+      if (r->repair_pass && rp.waves.size() == 1 && rp.agg == AGG_GENERAL) {
         // numGroupsLimit was reachable: if some key was refused (device-side check), zero the aggregates (keys and counters
         // stay) and aggregate the matches again in lookup-only mode, see pb_hash_slot
         const uint64_t skip16 = (((uint64_t)PB_COUNTERS_PER_TABLE * 8 * r->tables.size() + 255) & ~(uint64_t)255) / 16;
@@ -1567,8 +1559,7 @@ static int enqueue_all(pb_result_s* r, const std::vector<cudaEvent_t>* seg_wait)
                                                              w.dq.any_limit);
         DevQuery dq2 = w.dq;
         dq2.phase = 2;
-        if (rp.agg_kind == 2) pb_agg_kernel<4><<<w.grid_agg, PB_NTHREADS, rp.smem_agg, st>>>(dq2);
-        else pb_agg_kernel<6><<<w.grid_agg, PB_NTHREADS, rp.smem_agg, st>>>(dq2);
+        pb_agg_kernel<6><<<w.grid_agg, PB_NTHREADS, rp.smem_agg, st>>>(dq2);
         r->launches += 2;
         CU(cudaGetLastError());
       }
@@ -1657,215 +1648,256 @@ static int replay_plan(pb_result_s* r, const pb_query_desc* q) {
   return finish_finalize(r);
 }
 
-// One device's part of a query: every segment of `g` lives on g->ctx.  Leaves the tables on the device when
-// PB_Q_DEFER_FINALIZE is set; otherwise merges across ranks (PB_Q_ALL_RANKS) and finalizes.
-static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, const pb_query_desc* q, pb_result_handle* out) {
-  int rc = PB_OK;
-  Context* ctx = g->ctx;
-  const int n_segs = (int)g->segs.size();
-  const int nG = q->num_group_by, nA = q->num_aggregations;
+// ------------------------------------------------------------------------------------------------
+// planning: the stages of exec_single
+// ------------------------------------------------------------------------------------------------
+// What one exec_single call has worked out so far, handed from stage to stage (host side only)
+struct Plan {
+  pb_group_s* g = nullptr; const pb_segment_query* sqs = nullptr; const pb_query_desc* q = nullptr;
+  pb_result_s* r = nullptr; Context* ctx = nullptr; cudaStream_t st = nullptr;
+  int n_segs = 0, nG = 0, nA = 0, nF = 0, n_tables = 0;
+  bool combine = false, in_place = false;
+  // ---- columns (stage_inputs) ----
+  std::vector<std::vector<int>> gcol, acol;          // per segment: column of every group-by key / aggregation input (-1: COUNT)
+  bool any_raw_key = false;
+  std::vector<const RowGroup*> seg_rg;               // row group the gathers of each segment read from (nullptr: the columns themselves)
+  std::vector<std::vector<char>> cand_leaf;          // per filter node: scan leaf evaluated on candidates (DevLeaf::gather)
+  std::vector<std::vector<double>> cand_frac;
+  std::vector<cudaEvent_t> seg_wait;                 // staging events this call's kernels must wait for
+  int n_pending = 0;
+  std::vector<GlobalDict*> gdict, adict;             // combined mode: global dictionaries of the keys / DISTINCTCOUNT inputs
+  // ---- tables (plan_table_mode, alloc_tables) ----
+  std::vector<uint64_t> dc_words;
+  std::vector<char> dc_raw;                          // DISTINCTCOUNT on a raw column: a (slot, value) set instead of a dictId bitset
+  size_t zero_bytes = 0, ff_bytes = 0, mm_elems = 0, aux_bytes = 0, any_limit_off = 0;
+  uint8_t *d_zero = nullptr, *d_ff = nullptr, *d_aux = nullptr;
+  // ---- descriptors ----
+  Arena ar;
+  DevQuery* hq = nullptr; DevSegQuery* hsegs = nullptr;   // host views of the arena
+  DevSegQuery* d_segs = nullptr; DevTable* d_tabs = nullptr;
+  uint32_t* d_bitmaps = nullptr; size_t bm_off = 0;
+  std::vector<DevExpandItem> expand_items;         // one per inverted-index bitmap / per sorted-index range list
+  int slot_bits_max[PB_MAX_SCAN_SLOTS] = {0};
+  int set_cache_max = 0, n_slots_max = 0;
+  bool any_cand_leaf = false;
+  DevRowSeg* h_row_segs = nullptr; const DevRowSeg* d_row_segs = nullptr; int rows_rw = 0;
+  int U = 2; size_t stage_bytes = 0;
+  uint64_t n_chunks = 0, n_docs_total = 0;
+  bool match_all = true;
+  size_t st_rep_bytes = 0; int st_replicas = 0;     // CTA-private shared-memory table (pb_agg_smem_kernel)
+  uint32_t* d_match_list = nullptr;
+  const unsigned long long* d_head = nullptr;
+  const DevLaneWeights* d_lane_w = nullptr;
+  const DevExpandItem* d_expand_items = nullptr;
+};
+
+// Argument checks that need no segment: all of them run before the plan-cache lookup
+static int validate_query(pb_group_s* g, const pb_segment_query* sqs, const pb_query_desc* q) {
+  const int nG = q->num_group_by, nA = q->num_aggregations, nF = q->num_agg_filters;
   if (nG < 0 || nG > PB_MAX_GROUP_BY) return fail(PB_ERR_UNSUPPORTED, "%d group-by columns (max %d)", nG, PB_MAX_GROUP_BY);
   if (nA <= 0 || nA > PB_MAX_AGGS) return fail(PB_ERR_UNSUPPORTED, "%d aggregations (max %d)", nA, PB_MAX_AGGS);
-  const bool combine = (q->flags & PB_Q_COMBINE) != 0;
-  const bool in_place = (q->flags & PB_Q_GATHER_IN_PLACE) != 0;
-  const int n_tables = combine ? 1 : n_segs;
-  const int nF = q->num_agg_filters;
-  const bool count_all = (q->flags & PB_Q_NULL_HANDLING) != 0;
   if (nF < 0 || nF > PB_MAX_AGG_FILTERS) return fail(PB_ERR_UNSUPPORTED, "%d FILTER clauses (max %d)", nF, PB_MAX_AGG_FILTERS);
   if (nF > 0) {
     if (!q->agg_filter_of) return fail(PB_ERR_INVALID, "agg_filter_of missing");
     for (int a = 0; a < nA; a++) if (q->agg_filter_of[a] < -1 || q->agg_filter_of[a] >= nF) return fail(PB_ERR_INVALID, "aggregation %d: bad FILTER clause index", a);
-    for (int si = 0; si < n_segs; si++) if (!sqs[si].agg_filters || !sqs[si].agg_filter_nodes) return fail(PB_ERR_INVALID, "segment %d: FILTER clause programs missing", si);
+    for (int si = 0; si < (int)g->segs.size(); si++) if (!sqs[si].agg_filters || !sqs[si].agg_filter_nodes) return fail(PB_ERR_INVALID, "segment %d: FILTER clause programs missing", si);
   }
-
-  // ---- plan cache: the same query over the same segments again -> replay its parked plan ----
-  std::string sig;
-  const bool try_cache = plan_cache_enabled() && !(q->flags & (PB_Q_DEFER_FINALIZE | PB_Q_GATHER_IN_PLACE));
-  if (try_cache) {
-    sig = plan_signature(g, sqs, q);
-    if (pb_result_s* p = plan_take(g, sig)) {
-      if ((rc = replay_plan(p, q))) { free_result(p); return rc; }
-      *out = p;
-      return PB_OK;
-    }
-  }
-  std::unique_ptr<pb_result_s, void (*)(pb_result_s*)> R(new pb_result_s(), free_result);
-  pb_result_s* r = R.get();
-  r->group = g; r->n_gb = nG; r->n_aggs = nA; r->combine = combine; r->ctx = ctx;
-  if ((rc = stream_set_acquire(ctx, &r->sset))) return rc;
-  r->stream = r->sset.stream;
-  cudaStream_t st = r->stream;
-  r->ev0 = r->sset.ev[0]; r->ev1 = r->sset.ev[1]; r->evm = r->sset.ev[2]; r->ev2 = r->sset.ev[3]; r->ev3 = r->sset.ev[4];
-  for (int j = 0; j < nG; j++) r->gb_names.push_back(q->group_by_columns[j]);
   for (int a = 0; a < nA; a++) {
-    r->agg_op.push_back(q->aggregations[a].op);
-    r->agg_cols.push_back(q->aggregations[a].column ? q->aggregations[a].column : "");
     if (q->aggregations[a].op < PB_AGG_COUNT || q->aggregations[a].op > PB_AGG_DISTINCTCOUNT) return fail(PB_ERR_UNSUPPORTED, "aggregation op %d", q->aggregations[a].op);
     if (q->aggregations[a].op != PB_AGG_COUNT && !q->aggregations[a].column) return fail(PB_ERR_INVALID, "aggregation %d needs a column", a);
   }
+  return PB_OK;
+}
 
-  double t_prev = now_us();
-  auto lap = [&](int i) { double t = now_us(); r->host_us[i] += t - t_prev; t_prev = t; };
-  // ---- resolve columns, stage what is needed ----
-  std::vector<std::vector<int>> gcol(n_segs, std::vector<int>(nG)), acol(n_segs, std::vector<int>(nA, -1));
-  bool any_raw_key = false;
-  cudaStream_t cs = ctx->copy_stream;
-  std::vector<cudaEvent_t> seg_wait(n_segs, nullptr);   // staging events this call's kernels must wait for
-  int n_pending = 0;
-  static const bool row_groups_on = []() { const char* e = getenv("PB_ROW_GROUPS"); return !e || atoi(e) != 0; }();
-  std::vector<const RowGroup*> seg_rg(n_segs, nullptr);  // row group the gathers of each segment read from (nullptr: the columns themselves)
-  std::vector<std::vector<char>> cand_leaf(n_segs);     // per filter node: scan leaf evaluated on candidates (DevLeaf::gather)
-  std::vector<std::vector<double>> cand_frac(n_segs);
-  for (int si = 0; si < n_segs; si++) plan_candidate_leaves(g->segs[si], sqs[si], cand_leaf[si], cand_frac[si]);
-  for (int si = 0; si < n_segs; si++) {
-    pb_segment_s* s = g->segs[si];
-    std::lock_guard<std::mutex> lk(s->mu);
-    s->inflight++; r->pinned_segments = si + 1;
-    { std::lock_guard<std::mutex> lk2(ctx->mu); s->last_used = ++ctx->lru_clock; }
-    // PB_Q_GATHER_IN_PLACE, per column: a gathered value costs one 32-byte PCIe read = 32 B payload + ~24 B of TLP
-    // overhead of link time (PCIe Gen5: the cold query is link-bound and each in-place value costs ~56 streamed
-    // bytes); copying the column costs bits/8 bytes per doc.  Gather in place only where that is cheaper:
-    // expected matches x 56 B < column bytes.
-    // (PB_IN_PLACE_COST overrides the 56 B; 0 = always gather: used by the tests to reach every code path.)
-    const double sel = in_place ? estimate_selectivity(s, sqs[si]) : 1.0;
-    double gather_cost = 56.0;
-    if (in_place) if (const char* e = getenv("PB_IN_PLACE_COST")) gather_cost = atof(e);
-    auto gather_ok = [&](const Column& c) {
-      if (!in_place) return false;
-      const double col_bytes_per_doc = c.has_dict ? c.bits / 8.0 : (double)c.raw_width;
-      return sel * gather_cost < col_bytes_per_doc;
+// PB_Q_GATHER_IN_PLACE, per column: a gathered value costs one 32-byte PCIe read = 32 B payload + ~24 B of TLP overhead of
+// link time (PCIe Gen5: the cold query is link-bound and each in-place value costs ~56 streamed bytes, PB_IN_PLACE_COST);
+// copying the column costs bits/8 bytes per doc.  Gather in place only where that is cheaper: frac = expected fraction of
+// the docs whose value is read.
+static bool cheaper_in_place(const Column& c, double frac, double gather_cost) {
+  const double col_bytes_per_doc = c.has_dict ? c.bits / 8.0 : (double)c.raw_width;
+  return frac * gather_cost < col_bytes_per_doc;
+}
+
+// Stage the columns of one filter program: the main filter (clause < 0) or FILTER clause `clause`.  in_place(n, c): the scan
+// leaf n may read column c where it lies instead of from a staged copy.
+template <class InPlace>
+static int stage_filter_columns(pb_segment_s* s, const pb_filter_node* nodes, int n_nodes, int clause, cudaStream_t cs, InPlace in_place) {
+  for (int n = 0; n < n_nodes; n++) {
+    const pb_filter_node& fn = nodes[n];
+    if (fn.kind < PB_F_SCAN_DICT_RANGE || fn.kind > PB_F_INVERTED) continue;
+    auto bad = [&](const char* what) {
+      return clause < 0 ? fail(PB_ERR_INVALID, "filter node %d: %s", n, what) : fail(PB_ERR_INVALID, "FILTER clause %d node %d: %s", clause, n, what);
     };
-    for (int j = 0; j < nG; j++) {
-      int ci = find_col(s, q->group_by_columns[j]);
-      if (ci < 0) return fail(PB_ERR_INVALID, "segment %s: no column %s", s->name.c_str(), q->group_by_columns[j]);
-      gcol[si][j] = ci;
-      Column& c = s->cols[ci];
-      if (!c.has_dict) any_raw_key = true;
-      if ((rc = stage_column(s, c, true, false, false, cs, !combine, gather_ok(c)))) return rc;
-    }
-    for (int a = 0; a < nA; a++) {
-      if (q->aggregations[a].op == PB_AGG_COUNT) continue;
-      int ci = find_col(s, q->aggregations[a].column);
-      if (ci < 0) return fail(PB_ERR_INVALID, "segment %s: no column %s", s->name.c_str(), q->aggregations[a].column);
-      acol[si][a] = ci;
-      Column& c = s->cols[ci];
-      if (q->aggregations[a].op == PB_AGG_DISTINCTCOUNT) {
-        if (!c.has_dict && c.type == PB_STRING) return fail(PB_ERR_UNSUPPORTED, "DISTINCTCOUNT on raw STRING column %s", c.name.c_str());
-        if ((rc = stage_column(s, c, true, false, false, cs, false, gather_ok(c)))) return rc;
-      } else {
-        if (c.type == PB_STRING) return fail(PB_ERR_UNSUPPORTED, "numeric aggregation on STRING column %s", c.name.c_str());
-        if ((rc = stage_column(s, c, true, true, false, cs, false, gather_ok(c)))) return rc;
-      }
-    }
-    const pb_segment_query& sq = sqs[si];
-    if (sq.num_filter_nodes > PB_MAX_NODES) return fail(PB_ERR_UNSUPPORTED, "filter has %d nodes (max %d)", sq.num_filter_nodes, PB_MAX_NODES);
-    for (int n = 0; n < sq.num_filter_nodes; n++) {
-      const pb_filter_node& fn = sq.filter[n];
-      if (fn.kind >= PB_F_SCAN_DICT_RANGE && fn.kind <= PB_F_INVERTED) {
-        if (fn.column < 0 || fn.column >= (int)s->cols.size()) return fail(PB_ERR_INVALID, "filter node %d: bad column", n);
-        Column& c = s->cols[fn.column];
-        bool inv = fn.kind == PB_F_INVERTED;
-        if ((fn.kind == PB_F_SCAN_DICT_RANGE || fn.kind == PB_F_SCAN_DICT_SET) && !c.has_dict) return fail(PB_ERR_INVALID, "filter node %d: dictionary scan on raw column", n);
-        if ((fn.kind == PB_F_SCAN_RAW_RANGE || fn.kind == PB_F_SCAN_RAW_SET) && c.has_dict) return fail(PB_ERR_INVALID, "filter node %d: raw scan on dictionary column", n);
-        // a leaf that runs on candidates only reads the rows that reach it: cold segments can leave its column in host memory
-        bool leaf_in_place = false;
-        if (in_place && !inv && cand_leaf[si][n]) {
-          const double col_bytes_per_doc = c.has_dict ? c.bits / 8.0 : (double)c.raw_width;
-          leaf_in_place = cand_frac[si][n] * gather_cost < col_bytes_per_doc;
-        }
-        if ((rc = stage_column(s, c, !inv, false, inv, cs, false, leaf_in_place))) return rc;
-      }
-    }
-    // FILTER(WHERE ...) clauses: their leaves are tested per matching doc by the aggregation kernel (gathers)
-    for (int f = 0; f < nF; f++) {
-      if (sq.agg_filter_nodes[f] < 0 || sq.agg_filter_nodes[f] > PB_MAX_AF_NODES) return fail(PB_ERR_UNSUPPORTED, "FILTER clause %d has %d nodes (max %d)", f, sq.agg_filter_nodes[f], PB_MAX_AF_NODES);
-      for (int n = 0; n < sq.agg_filter_nodes[f]; n++) {
-        const pb_filter_node& fn = sq.agg_filters[f][n];
-        if (fn.kind >= PB_F_SCAN_DICT_RANGE && fn.kind <= PB_F_INVERTED) {
-          if (fn.column < 0 || fn.column >= (int)s->cols.size()) return fail(PB_ERR_INVALID, "FILTER clause %d node %d: bad column", f, n);
-          Column& c = s->cols[fn.column];
-          bool inv = fn.kind == PB_F_INVERTED;
-          if ((fn.kind == PB_F_SCAN_DICT_RANGE || fn.kind == PB_F_SCAN_DICT_SET) && !c.has_dict) return fail(PB_ERR_INVALID, "FILTER clause %d node %d: dictionary scan on raw column", f, n);
-          if ((fn.kind == PB_F_SCAN_RAW_RANGE || fn.kind == PB_F_SCAN_RAW_SET) && c.has_dict) return fail(PB_ERR_INVALID, "FILTER clause %d node %d: raw scan on dictionary column", f, n);
-          if ((rc = stage_column(s, c, !inv, false, inv, cs, false, !inv && gather_ok(c)))) return rc;
-        }
-      }
-    }
-    // ---- row group: the dictionary columns this query gathers per matching doc, side by side in one row ----
-    if (row_groups_on && !in_place) {
-      const double sel_rg = estimate_selectivity(s, sq);
-      if (sel_rg <= 0.5) {
-        std::vector<std::pair<int, int>> want;      // (column, form): 0 = dictId, 1 = decoded value (numeric aggregation inputs)
-        auto add = [&](int ci, int form) {
-          if (ci < 0 || !s->cols[ci].has_dict || !s->cols[ci].fwd_staged) return;
-          if (std::find(want.begin(), want.end(), std::make_pair(ci, form)) == want.end()) want.push_back({ci, form});
-        };
-        for (int j = 0; j < nG; j++) add(gcol[si][j], 0);
-        for (int a = 0; a < nA; a++) {
-          if (acol[si][a] < 0) continue;
-          Column& c = s->cols[acol[si][a]];
-          const bool decoded = q->aggregations[a].op != PB_AGG_DISTINCTCOUNT && c.has_dict && c.type != PB_STRING;
-          if (decoded && !c.native_staged && (rc = stage_column(s, c, false, false, false, cs, true, false))) return rc;   // the build reads the native dictionary
-          add(acol[si][a], decoded ? 1 : 0);
-        }
-        for (int n = 0; n < sq.num_filter_nodes; n++)
-          if (cand_leaf[si][n] && (sq.filter[n].kind == PB_F_SCAN_DICT_RANGE || sq.filter[n].kind == PB_F_SCAN_DICT_SET)) add(sq.filter[n].column, 0);
-        for (int f = 0; f < nF; f++)
-          for (int n = 0; n < sq.agg_filter_nodes[f]; n++)
-            if (sq.agg_filters[f][n].kind == PB_F_SCAN_DICT_RANGE || sq.agg_filters[f][n].kind == PB_F_SCAN_DICT_SET) add(sq.agg_filters[f][n].column, 0);
-        std::sort(want.begin(), want.end());
-        seg_rg[si] = row_group_for(s, want, cs);
-      }
-    }
-    if (s->device_bytes != s->accounted_bytes) {
-      std::lock_guard<std::mutex> lk2(ctx->mu);
-      ctx->staged_bytes += s->device_bytes - s->accounted_bytes;
-      s->accounted_bytes = s->device_bytes;
-    }
-    // order this (and every later) query's kernels after the copies just enqueued for the segment
-    if (s->stage_dirty) {
-      if (!s->staged_ev) CU(cudaEventCreateWithFlags(&s->staged_ev, cudaEventDisableTiming));
-      CU(cudaEventRecord(s->staged_ev, cs));
-      s->stage_dirty = false; s->staged_pending = true;
-    }
-    if (s->staged_pending) {
-      if (cudaEventQuery(s->staged_ev) == cudaSuccess) s->staged_pending = false;
-      else { seg_wait[si] = s->staged_ev; n_pending++; }
-      cudaGetLastError();   // cudaErrorNotReady is not an error
-    }
+    if (fn.column < 0 || fn.column >= (int)s->cols.size()) return bad("bad column");
+    Column& c = s->cols[fn.column];
+    const bool inv = fn.kind == PB_F_INVERTED;
+    if ((fn.kind == PB_F_SCAN_DICT_RANGE || fn.kind == PB_F_SCAN_DICT_SET) && !c.has_dict) return bad("dictionary scan on raw column");
+    if ((fn.kind == PB_F_SCAN_RAW_RANGE || fn.kind == PB_F_SCAN_RAW_SET) && c.has_dict) return bad("raw scan on dictionary column");
+    const int rc = stage_column(s, c, !inv, false, inv, cs, false, !inv && in_place(n, c));
+    if (rc) return rc;
   }
+  return PB_OK;
+}
 
-  enforce_cache_limit(ctx);      // this call's segments are pinned: only others can go
-
-  // ---- global dictionaries (combined mode) ----
-  std::vector<GlobalDict*> gdict(nG, nullptr), adict(nA, nullptr);
-  if (combine) {
-    for (int j = 0; j < nG; j++) {
-      if (!g->segs[0]->cols[gcol[0][j]].has_dict) continue;
-      if ((rc = get_global_dict(g, q->group_by_columns[j], &gdict[j]))) return rc;
-    }
-    for (int a = 0; a < nA; a++)
-      if (q->aggregations[a].op == PB_AGG_DISTINCTCOUNT && g->segs[0]->cols[acol[0][a]].has_dict &&
-          (rc = get_global_dict(g, q->aggregations[a].column, &adict[a]))) return rc;
+// Row group of segment si: the dictionary columns this query gathers per matching doc, side by side in one row
+static int pick_row_group(Plan& P, int si) {
+  static const bool row_groups_on = []() { const char* e = getenv("PB_ROW_GROUPS"); return !e || atoi(e) != 0; }();
+  pb_segment_s* s = P.g->segs[si];
+  const pb_segment_query& sq = P.sqs[si];
+  if (!row_groups_on || P.in_place || estimate_selectivity(s, sq) > 0.5) return PB_OK;
+  std::vector<std::pair<int, int>> want;      // (column, form): 0 = dictId, 1 = decoded value (numeric aggregation inputs)
+  auto add = [&](int ci, int form) {
+    if (ci < 0 || !s->cols[ci].has_dict || !s->cols[ci].fwd_staged) return;
+    if (std::find(want.begin(), want.end(), std::make_pair(ci, form)) == want.end()) want.push_back({ci, form});
+  };
+  for (int j = 0; j < P.nG; j++) add(P.gcol[si][j], 0);
+  for (int a = 0; a < P.nA; a++) {
+    if (P.acol[si][a] < 0) continue;
+    Column& c = s->cols[P.acol[si][a]];
+    const bool decoded = P.q->aggregations[a].op != PB_AGG_DISTINCTCOUNT && c.has_dict && c.type != PB_STRING;
+    int rc;
+    if (decoded && !c.native_staged && (rc = stage_column(s, c, false, false, false, P.ctx->copy_stream, true, false))) return rc;   // the build reads the native dictionary
+    add(P.acol[si][a], decoded ? 1 : 0);
   }
+  for (int n = 0; n < sq.num_filter_nodes; n++)
+    if (P.cand_leaf[si][n] && (sq.filter[n].kind == PB_F_SCAN_DICT_RANGE || sq.filter[n].kind == PB_F_SCAN_DICT_SET)) add(sq.filter[n].column, 0);
+  for (int f = 0; f < P.nF; f++)
+    for (int n = 0; n < sq.agg_filter_nodes[f]; n++)
+      if (sq.agg_filters[f][n].kind == PB_F_SCAN_DICT_RANGE || sq.agg_filters[f][n].kind == PB_F_SCAN_DICT_SET) add(sq.agg_filters[f][n].column, 0);
+  std::sort(want.begin(), want.end());
+  P.seg_rg[si] = row_group_for(s, want, P.ctx->copy_stream);
+  return PB_OK;
+}
 
-  lap(0);
-  // ---- table mode and layout ----
-  r->tables.resize(n_tables);
-  int table_mode = nG == 0 ? T_KEYLESS : T_DENSE;
-  int key_words = 1;
+// Pin segment si, resolve the columns the query names and stage what its kernels read, build its row group, and record
+// the staging event its kernels must wait for
+static int stage_segment(Plan& P, int si) {
+  int rc;
+  pb_segment_s* s = P.g->segs[si];
+  const pb_query_desc* q = P.q;
+  Context* ctx = P.ctx;
+  cudaStream_t cs = ctx->copy_stream;
+  std::lock_guard<std::mutex> lk(s->mu);
+  s->inflight++; P.r->pinned_segments = si + 1;
+  { std::lock_guard<std::mutex> lk2(ctx->mu); s->last_used = ++ctx->lru_clock; }
+  // (PB_IN_PLACE_COST overrides the cost of an in-place value; 0 = always gather: used by the tests to reach every code path.)
+  const double sel = P.in_place ? estimate_selectivity(s, P.sqs[si]) : 1.0;
+  double gather_cost = 56.0;
+  if (P.in_place) if (const char* e = getenv("PB_IN_PLACE_COST")) gather_cost = atof(e);
+  auto gather_ok = [&](const Column& c) { return P.in_place && cheaper_in_place(c, sel, gather_cost); };
+  for (int j = 0; j < P.nG; j++) {
+    int ci = find_col(s, q->group_by_columns[j]);
+    if (ci < 0) return fail(PB_ERR_INVALID, "segment %s: no column %s", s->name.c_str(), q->group_by_columns[j]);
+    P.gcol[si][j] = ci;
+    Column& c = s->cols[ci];
+    if (!c.has_dict) P.any_raw_key = true;
+    if ((rc = stage_column(s, c, true, false, false, cs, !P.combine, gather_ok(c)))) return rc;
+  }
+  for (int a = 0; a < P.nA; a++) {
+    if (q->aggregations[a].op == PB_AGG_COUNT) continue;
+    int ci = find_col(s, q->aggregations[a].column);
+    if (ci < 0) return fail(PB_ERR_INVALID, "segment %s: no column %s", s->name.c_str(), q->aggregations[a].column);
+    P.acol[si][a] = ci;
+    Column& c = s->cols[ci];
+    const bool numeric = q->aggregations[a].op != PB_AGG_DISTINCTCOUNT;
+    if (!numeric && !c.has_dict && c.type == PB_STRING) return fail(PB_ERR_UNSUPPORTED, "DISTINCTCOUNT on raw STRING column %s", c.name.c_str());
+    if (numeric && c.type == PB_STRING) return fail(PB_ERR_UNSUPPORTED, "numeric aggregation on STRING column %s", c.name.c_str());
+    if ((rc = stage_column(s, c, true, numeric, false, cs, false, gather_ok(c)))) return rc;
+  }
+  const pb_segment_query& sq = P.sqs[si];
+  if (sq.num_filter_nodes > PB_MAX_NODES) return fail(PB_ERR_UNSUPPORTED, "filter has %d nodes (max %d)", sq.num_filter_nodes, PB_MAX_NODES);
+  // a leaf that runs on candidates only reads the rows that reach it: cold segments can leave its column in host memory
+  auto leaf_in_place = [&](int n, const Column& c) { return P.in_place && P.cand_leaf[si][n] && cheaper_in_place(c, P.cand_frac[si][n], gather_cost); };
+  if ((rc = stage_filter_columns(s, sq.filter, sq.num_filter_nodes, -1, cs, leaf_in_place))) return rc;
+  // FILTER(WHERE ...) clauses: their leaves are tested per matching doc by the aggregation kernel (gathers)
+  for (int f = 0; f < P.nF; f++) {
+    if (sq.agg_filter_nodes[f] < 0 || sq.agg_filter_nodes[f] > PB_MAX_AF_NODES) return fail(PB_ERR_UNSUPPORTED, "FILTER clause %d has %d nodes (max %d)", f, sq.agg_filter_nodes[f], PB_MAX_AF_NODES);
+    if ((rc = stage_filter_columns(s, sq.agg_filters[f], sq.agg_filter_nodes[f], f, cs, [&](int, const Column& c) { return gather_ok(c); }))) return rc;
+  }
+  if ((rc = pick_row_group(P, si))) return rc;
+  if (s->device_bytes != s->accounted_bytes) {
+    std::lock_guard<std::mutex> lk2(ctx->mu);
+    ctx->staged_bytes += s->device_bytes - s->accounted_bytes;
+    s->accounted_bytes = s->device_bytes;
+  }
+  // order this (and every later) query's kernels after the copies just enqueued for the segment
+  if (s->stage_dirty) {
+    if (!s->staged_ev) CU(cudaEventCreateWithFlags(&s->staged_ev, cudaEventDisableTiming));
+    CU(cudaEventRecord(s->staged_ev, cs));
+    s->stage_dirty = false; s->staged_pending = true;
+  }
+  if (s->staged_pending) {
+    if (cudaEventQuery(s->staged_ev) == cudaSuccess) s->staged_pending = false;
+    else { P.seg_wait[si] = s->staged_ev; P.n_pending++; }
+    cudaGetLastError();   // cudaErrorNotReady is not an error
+  }
+  return PB_OK;
+}
+
+// Stage every segment, enforce the segment cache limit, and get the global dictionaries (combined mode)
+static int stage_inputs(Plan& P) {
+  int rc;
+  const int n_segs = P.n_segs;
+  P.gcol.assign(n_segs, std::vector<int>(P.nG));
+  P.acol.assign(n_segs, std::vector<int>(P.nA, -1));
+  P.seg_wait.assign(n_segs, nullptr);
+  P.seg_rg.assign(n_segs, nullptr);
+  P.cand_leaf.resize(n_segs); P.cand_frac.resize(n_segs);
+  for (int si = 0; si < n_segs; si++) plan_candidate_leaves(P.g->segs[si], P.sqs[si], P.cand_leaf[si], P.cand_frac[si]);
+  for (int si = 0; si < n_segs; si++) if ((rc = stage_segment(P, si))) return rc;
+
+  enforce_cache_limit(P.ctx);      // this call's segments are pinned: only others can go
+
+  P.gdict.assign(P.nG, nullptr); P.adict.assign(P.nA, nullptr);
+  if (P.combine) {
+    const pb_segment_s* s0 = P.g->segs[0];
+    for (int j = 0; j < P.nG; j++) {
+      if (!s0->cols[P.gcol[0][j]].has_dict) continue;
+      if ((rc = get_global_dict(P.g, P.q->group_by_columns[j], &P.gdict[j]))) return rc;
+    }
+    for (int a = 0; a < P.nA; a++)
+      if (P.q->aggregations[a].op == PB_AGG_DISTINCTCOUNT && s0->cols[P.acol[0][a]].has_dict &&
+          (rc = get_global_dict(P.g, P.q->aggregations[a].column, &P.adict[a]))) return rc;
+  }
+  return PB_OK;
+}
+
+static uint64_t slots_of(const Plan& P, const TableMeta& tm) { return tm.capacity + (P.r->table_mode == T_HASH ? 1 : 0); }
+static uint64_t table_docs(const Plan& P, const TableMeta& tm) {
+  uint64_t docs = 0;
+  for (int si : tm.seg_idx) docs += (uint64_t)P.g->segs[si]->num_docs;
+  return docs;
+}
+// COUNT / AVG under a FILTER clause (every aggregation under one with PB_Q_NULL_HANDLING) keeps its own row count
+static bool has_fcnt(const pb_query_desc* q, int a) {
+  const int op = q->aggregations[a].op;
+  return q->num_agg_filters > 0 && q->agg_filter_of[a] >= 0 && (op == PB_AGG_COUNT || op == PB_AGG_AVG || (q->flags & PB_Q_NULL_HANDLING));
+}
+
+// Table mode (keyless / dense / hash), capacities and key layout, the ORDER BY trim, first-doc tracking and the
+// DISTINCTCOUNT representations
+static int plan_table_mode(Plan& P) {
+  pb_result_s* r = P.r;
+  const pb_query_desc* q = P.q;
+  const int nG = P.nG, nA = P.nA;
+  r->tables.resize(P.n_tables);
+  for (int t = 0; t < P.n_tables; t++) {
+    TableMeta& tm = r->tables[t];
+    if (P.combine) for (int si = 0; si < P.n_segs; si++) tm.seg_idx.push_back(si); else tm.seg_idx.push_back(t);
+  }
+  r->table_mode = nG == 0 ? T_KEYLESS : T_DENSE;
   if (nG > 0) {
-    for (int t = 0; t < n_tables; t++) {
+    for (int t = 0; t < P.n_tables; t++) {
       TableMeta& tm = r->tables[t];
-      int si0 = combine ? 0 : t;
+      int si0 = P.combine ? 0 : t;
       tm.cards.resize(nG); tm.shifts.resize(nG); tm.widths.resize(nG);
       unsigned __int128 prod = 1;
       int total_bits = 0;
       for (int j = 0; j < nG; j++) {
-        const Column& c = g->segs[si0]->cols[gcol[si0][j]];
+        const Column& c = P.g->segs[si0]->cols[P.gcol[si0][j]];
         int64_t card; int width;
         if (c.has_dict) {
-          card = combine ? gdict[j]->n : c.card;
+          card = P.combine ? P.gdict[j]->n : c.card;
           width = 1; while ((1ll << width) < card) width++;
         } else {
           card = -1;
@@ -1875,33 +1907,25 @@ static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, c
         tm.cards[j] = card; tm.widths[j] = width; tm.shifts[j] = total_bits; total_bits += width;
         if (card > 0 && prod <= ((unsigned __int128)1 << 70)) prod *= (unsigned __int128)card;
       }
-      bool dense_ok = !any_raw_key && prod <= PB_DENSE_MAX;
+      bool dense_ok = !P.any_raw_key && prod <= PB_DENSE_MAX;
       if (!dense_ok) {
         if (total_bits > 128) return fail(PB_ERR_UNSUPPORTED, "group key needs %d bits (> 128): decline to the CPU plan", total_bits);
-        if (total_bits > 64) key_words = 2;
-        table_mode = T_HASH;
+        if (total_bits > 64) r->key_words = 2;
+        r->table_mode = T_HASH;
       }
       tm.capacity = dense_ok ? (uint64_t)prod : 0;
     }
   }
-  if (table_mode == T_HASH) {
-    for (int t = 0; t < n_tables; t++) {
-      TableMeta& tm = r->tables[t];
-      uint64_t docs = 0;
-      if (combine) for (auto* s : g->segs) docs += (uint64_t)s->num_docs; else docs = (uint64_t)g->segs[t]->num_docs;
-      uint64_t want = std::min<uint64_t>((uint64_t)std::max(1, q->num_groups_limit), std::max<uint64_t>(docs, 1));
+  if (r->table_mode == T_HASH) {
+    for (auto& tm : r->tables) {
+      uint64_t want = std::min<uint64_t>((uint64_t)std::max(1, q->num_groups_limit), std::max<uint64_t>(table_docs(P, tm), 1));
       uint64_t cap = 1024;
       while (cap < 2 * want) cap <<= 1;
       tm.capacity = cap;
     }
   }
-  if (table_mode == T_KEYLESS) for (auto& tm : r->tables) tm.capacity = 1;
-  r->table_mode = table_mode;
-  for (int t = 0; t < n_tables; t++) {
-    TableMeta& tm = r->tables[t];
-    tm.mode = table_mode;
-    if (combine) for (int si = 0; si < n_segs; si++) tm.seg_idx.push_back(si); else tm.seg_idx.push_back(t);
-  }
+  if (r->table_mode == T_KEYLESS) for (auto& tm : r->tables) tm.capacity = 1;
+  for (auto& tm : r->tables) tm.mode = r->table_mode;
 
   // ---- ORDER BY ... LIMIT trim requested? (first ORDER BY expression: a group-by column or a COUNT / SUM / MIN / MAX / AVG) ----
   if (q->num_order_by > 0 && q->order_by && q->trim_size > 0 && nG > 0) {
@@ -1912,130 +1936,120 @@ static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, c
     r->order0 = ob; r->trim_size = q->trim_size; r->trim_threshold = std::max(0, q->trim_threshold);
   }
 
-  // ---- device table arenas: [zero region][0xFF region][min/max region] ----
-  auto slots_of = [&](const TableMeta& tm) { return tm.capacity + (table_mode == T_HASH ? 1 : 0); };
-  size_t zero_bytes = 0, ff_bytes = 0, mm_elems = 0;
   // numGroupsLimit below the key space of a dense table: the reference creates groups first come first served in doc order
   // (IntMapBasedHolder); kept exact for per-segment tables (a merged table reports the superset and the flag, DESIGN.md §4.6)
-  bool track_first = false;
-  if (table_mode == T_DENSE && (!combine || n_segs == 1))
-    for (auto& tm : r->tables) if ((uint64_t)std::max(1, q->num_groups_limit) < tm.capacity) track_first = true;
-  r->track_first = track_first;
-  std::vector<uint64_t> dc_words(nA, 0);
-  std::vector<char> dc_raw(nA, 0);           // DISTINCTCOUNT on a raw column: a (slot, value) set instead of a dictId bitset
+  if (r->table_mode == T_DENSE && (!P.combine || P.n_segs == 1))
+    for (auto& tm : r->tables) if ((uint64_t)std::max(1, q->num_groups_limit) < tm.capacity) r->track_first = true;
+  P.dc_words.assign(nA, 0);
+  P.dc_raw.assign(nA, 0);
   for (int a = 0; a < nA; a++)
-    if (q->aggregations[a].op == PB_AGG_DISTINCTCOUNT && !g->segs[0]->cols[acol[0][a]].has_dict) dc_raw[a] = 1;
+    if (q->aggregations[a].op == PB_AGG_DISTINCTCOUNT && !P.g->segs[0]->cols[P.acol[0][a]].has_dict) P.dc_raw[a] = 1;
   for (int a = 0; a < nA; a++)
-    if (q->aggregations[a].op == PB_AGG_DISTINCTCOUNT && !dc_raw[a]) {
+    if (q->aggregations[a].op == PB_AGG_DISTINCTCOUNT && !P.dc_raw[a]) {
       int64_t maxcard = 0;
-      if (combine) maxcard = adict[a]->n; else for (int si = 0; si < n_segs; si++) maxcard = std::max<int64_t>(maxcard, g->segs[si]->cols[acol[si][a]].card);
-      dc_words[a] = ((uint64_t)maxcard + 31) / 32;
+      if (P.combine) maxcard = P.adict[a]->n; else for (int si = 0; si < P.n_segs; si++) maxcard = std::max<int64_t>(maxcard, P.g->segs[si]->cols[P.acol[si][a]].card);
+      P.dc_words[a] = ((uint64_t)maxcard + 31) / 32;
     }
-  for (auto& tm : r->tables) {
-    uint64_t S = slots_of(tm);
-    zero_bytes += 8 * S;                                     // rowcnt
+  return PB_OK;
+}
+
+// The one walk over the table block's regions.  Zeroed region: [counters of every table | per table, 256-byte aligned: row
+// counts, FILTER-clause row counts, sums, distinct bitsets / counts]; the min/max region follows it in the same allocation;
+// hash keys, first docs and raw DISTINCTCOUNT value sets live in a separate 0xFF-filled one.  Called before the allocation
+// (P.d_zero null) to size the regions, and after it to point every DevTable (its counter cells too) and the cross-GPU spans
+// of table 0 into them.
+static int lay_out_tables(Plan& P) {
+  pb_result_s* r = P.r;
+  const pb_query_desc* q = P.q;
+  const int nA = P.nA;
+  long long* d_mm = P.d_zero && P.mm_elems ? reinterpret_cast<long long*>(P.d_zero + P.zero_bytes) : nullptr;
+  auto zp = [&](size_t off) -> void* { return P.d_zero ? P.d_zero + off : nullptr; };
+  auto fp = [&](size_t off) -> void* { return P.d_ff ? P.d_ff + off : nullptr; };
+  const size_t head = 8 * PB_COUNTERS_PER_TABLE * (size_t)P.n_tables;
+  const size_t tables_off = (head + 255) & ~(size_t)255;
+  size_t zo = tables_off, fo = 0, mo = 0;
+  for (int t = 0; t < P.n_tables; t++) {
+    TableMeta& tm = r->tables[t];
+    const uint64_t S = slots_of(P, tm);
+    DevTable& dt = tm.dev;
+    memset(&dt, 0, sizeof dt);
+    dt.mode = r->table_mode; dt.capacity = tm.capacity;
+    dt.rowcnt = static_cast<unsigned long long*>(zp(zo)); zo += 8 * S;
+    for (int a = 0; a < nA; a++)     // (u64, summed across GPUs with the row counts)
+      if (has_fcnt(q, a)) { dt.fcnt[a] = static_cast<unsigned long long*>(zp(zo)); zo += 8 * S; }
+    if (t == 0) { r->span_i64 = static_cast<unsigned long long*>(zp(0)); r->span_i64_n = (int64_t)(zo / 8); r->block_sum_off = (int64_t)zo; }
+    // sums first (one contiguous float64 span for the cross-GPU reduce), then the distinct bitsets
     for (int a = 0; a < nA; a++) {
       int op = q->aggregations[a].op;
-      if (nF > 0 && q->agg_filter_of[a] >= 0 && (op == PB_AGG_COUNT || op == PB_AGG_AVG || count_all)) zero_bytes += 8 * S;   // fcnt
-      if (op == PB_AGG_SUM || op == PB_AGG_AVG) zero_bytes += 8 * S;
-      if (op == PB_AGG_MIN || op == PB_AGG_MAX) mm_elems += S;
-      if (op == PB_AGG_DISTINCTCOUNT && !dc_raw[a]) zero_bytes += 4 * S * dc_words[a];
-      if (op == PB_AGG_DISTINCTCOUNT && dc_raw[a]) {
-        zero_bytes += 8 * S;                                   // dcnt
-        uint64_t docs = 0;
-        for (int si : tm.seg_idx) docs += (uint64_t)g->segs[si]->num_docs;
-        uint64_t cap = 1024;
-        while (cap < 2 * docs) cap <<= 1;                      // at most one entry per doc
-        if (cap > (1ull << 28)) return fail(PB_ERR_UNSUPPORTED, "DISTINCTCOUNT on raw column %s over %llu docs: value set too large", q->aggregations[a].column, (unsigned long long)docs);
-        tm.dset_cap.resize(nA, 0); tm.dset_cap[a] = cap;
-        ff_bytes += 16 * cap;
-      }
+      if (op == PB_AGG_SUM || op == PB_AGG_AVG) { dt.sum[a] = static_cast<double*>(zp(zo)); zo += 8 * S; }
     }
-    zero_bytes = (zero_bytes + 255) & ~(size_t)255;
-    if (table_mode == T_HASH) ff_bytes += (8 * S * (size_t)key_words + 15) & ~(size_t)15;      // (every piece of the 0xFF region starts 16-byte aligned: CAS.128)
-    if (track_first) ff_bytes += (4 * S + 15) & ~(size_t)15;
+    if (t == 0) { r->span_f64 = static_cast<double*>(zp((size_t)r->block_sum_off)); r->span_f64_n = (int64_t)((zo - (size_t)r->block_sum_off) / 8); r->block_dc_off = (int64_t)zo; }
+    for (int a = 0; a < nA; a++) {
+      int op = q->aggregations[a].op;
+      if (op == PB_AGG_DISTINCTCOUNT && !P.dc_raw[a]) { dt.dc_bits[a] = static_cast<uint32_t*>(zp(zo)); dt.dc_words[a] = P.dc_words[a]; zo += 4 * S * P.dc_words[a]; }
+      if (op == PB_AGG_DISTINCTCOUNT && P.dc_raw[a]) { dt.dcnt[a] = static_cast<unsigned long long*>(zp(zo)); zo += 8 * S; }
+      if (op == PB_AGG_MIN || op == PB_AGG_MAX) { dt.mm[a] = d_mm ? d_mm + mo : nullptr; mo += S; }
+    }
+    if (t == 0) { r->span_mm = d_mm; r->span_mm_n = (int64_t)mo; }
+    zo = (zo + 255) & ~(size_t)255;
+    // every piece of the 0xFF region starts 16-byte aligned (CAS.128)
+    if (r->table_mode == T_HASH) { dt.hkeys = static_cast<unsigned long long*>(fp(fo)); fo += (8 * S * (size_t)r->key_words + 15) & ~(size_t)15; dt.key_words = r->key_words; }
+    if (r->track_first) { dt.first_doc = static_cast<uint32_t*>(fp(fo)); fo += (4 * S + 15) & ~(size_t)15; }
+    for (int a = 0; a < nA; a++) {
+      if (!P.dc_raw[a]) continue;
+      const uint64_t docs = table_docs(P, tm);
+      uint64_t cap = 1024;
+      while (cap < 2 * docs) cap <<= 1;                      // at most one entry per doc
+      if (cap > (1ull << 28)) return fail(PB_ERR_UNSUPPORTED, "DISTINCTCOUNT on raw column %s over %llu docs: value set too large", q->aggregations[a].column, (unsigned long long)docs);
+      tm.dset_cap.resize(nA, 0); tm.dset_cap[a] = cap;
+      dt.dset[a] = static_cast<unsigned long long*>(fp(fo)); dt.dset_mask[a] = cap - 1; fo += 16 * cap;
+    }
+    if (!P.d_zero) continue;
+    unsigned long long* cnt = r->d_counters + (size_t)t * PB_COUNTERS_PER_TABLE;
+    dt.num_groups = reinterpret_cast<unsigned int*>(cnt + 0);
+    dt.limit_reached = reinterpret_cast<unsigned int*>(cnt + 1);
+    dt.any_limit = reinterpret_cast<unsigned int*>(P.d_aux + P.any_limit_off);
+    dt.docs_matched = cnt + 2;
+    dt.num_groups_limit = (uint32_t)std::max(1, q->num_groups_limit);
+    dt.limit_active = (uint64_t)dt.num_groups_limit < table_docs(P, tm) ? 1u : 0u;    // groups <= docs: an unreachable limit needs no tickets
   }
-  const size_t seg_stats_bytes = nF > 0 ? 8 * (size_t)(1 + PB_MAX_AGG_FILTERS) * (size_t)n_segs : 0;   // swim-lane statistics per segment
-  zero_bytes += 8 * PB_COUNTERS_PER_TABLE * (size_t)n_tables + 256;
+  // the zeroed region reserves 256 bytes beyond the counters and tables (its size is the block size the ranks compare)
+  const size_t zero_need = zo - tables_off + head + 256;
   // a group table may take at most a third of the device's HBM: the staged segments and the match list need the rest
-  if (zero_bytes > ctx->total_mem / 3) return fail(PB_ERR_UNSUPPORTED, "group table needs %zu bytes: decline to the CPU plan", zero_bytes);
-  uint8_t *d_zero = nullptr, *d_ff = nullptr; long long* d_mm = nullptr;
-  unsigned long long* d_seg_stats = nullptr;
+  if (zero_need > P.ctx->total_mem / 3) return fail(PB_ERR_UNSUPPORTED, "group table needs %zu bytes: decline to the CPU plan", zero_need);
+  P.zero_bytes = (zero_need + 255) & ~(size_t)255;
+  P.ff_bytes = fo; P.mm_elems = mo;
+  return PB_OK;
+}
+
+// Allocate the table block (lay_out_tables), its aux cells and the ORDER BY trim buffers, and point the tables into them
+static int alloc_tables(Plan& P) {
+  int rc;
+  pb_result_s* r = P.r;
+  cudaStream_t st = P.st;
+  if ((rc = lay_out_tables(P))) return rc;
   // one block: [zero region | min/max region] so that a cross-GPU merge can ship the whole table in one collective.  Its size
   // and layout depend on the query and the (global) dictionaries only -- never on how many segments this rank holds: the
   // per-wave match counters and per-segment swim-lane statistics live in an aux region behind it that is not shipped.
-  zero_bytes = (zero_bytes + 255) & ~(size_t)255;
-  const size_t mm_bytes = (8 * mm_elems + 255) & ~(size_t)255;
-  const size_t any_limit_off = 8 * PB_MAX_WAVES + seg_stats_bytes;   // query-wide "a key was refused" flag (hash tables)
-  const size_t thr_off = any_limit_off + 8;          // numGroupsLimit thresholds (one u32 per table), after the statistics
-  const size_t aux_bytes = (thr_off + (track_first ? 4 * (size_t)n_tables : 0) + 255) & ~(size_t)255;
-  CU(cudaMallocAsync((void**)&d_zero, zero_bytes + mm_bytes + aux_bytes + 16, st)); r->dev_allocs.push_back(d_zero);
-  if (ff_bytes) { CU(cudaMallocAsync((void**)&d_ff, ff_bytes + 16, st)); r->dev_allocs.push_back(d_ff); }
-  if (mm_elems) d_mm = reinterpret_cast<long long*>(d_zero + zero_bytes);
-  uint8_t* d_aux = d_zero + zero_bytes + mm_bytes;
-  r->d_first_thr = track_first ? reinterpret_cast<uint32_t*>(d_aux + thr_off) : nullptr;
-  r->block = d_zero; r->block_bytes = (int64_t)(zero_bytes + 8 * mm_elems);
-  r->block_mm_off = (int64_t)zero_bytes;
-
-  {
-    size_t zo = 0, fo = 0, mo = 0;
-    r->d_counters = reinterpret_cast<unsigned long long*>(d_zero);
-    zo += 8 * PB_COUNTERS_PER_TABLE * (size_t)n_tables;
-    if (seg_stats_bytes) d_seg_stats = reinterpret_cast<unsigned long long*>(d_aux + 8 * PB_MAX_WAVES);
-    r->d_seg_stats = d_seg_stats;
-    zo = (zo + 255) & ~(size_t)255;
-    for (int t = 0; t < n_tables; t++) {
-      TableMeta& tm = r->tables[t];
-      uint64_t S = slots_of(tm);
-      DevTable& dt = tm.dev;
-      memset(&dt, 0, sizeof dt);
-      dt.mode = table_mode; dt.capacity = tm.capacity;
-      dt.rowcnt = reinterpret_cast<unsigned long long*>(d_zero + zo); zo += 8 * S;
-      for (int a = 0; a < nA; a++) {   // row counts of COUNT / AVG with a FILTER clause (u64, summed across GPUs with the row counts)
-        int op = q->aggregations[a].op;
-        if (nF > 0 && q->agg_filter_of[a] >= 0 && (op == PB_AGG_COUNT || op == PB_AGG_AVG || count_all)) { dt.fcnt[a] = reinterpret_cast<unsigned long long*>(d_zero + zo); zo += 8 * S; }
-      }
-      if (t == 0) { r->span_i64 = r->d_counters; r->span_i64_n = (int64_t)((d_zero + zo - (uint8_t*)r->d_counters) / 8); }
-      // sums first (one contiguous float64 span for the cross-GPU reduce), then the distinct bitsets
-      if (t == 0) r->span_f64 = reinterpret_cast<double*>(d_zero + zo);
-      for (int a = 0; a < nA; a++) {
-        int op = q->aggregations[a].op;
-        if (op == PB_AGG_SUM || op == PB_AGG_AVG) { dt.sum[a] = reinterpret_cast<double*>(d_zero + zo); zo += 8 * S; }
-      }
-      if (t == 0) r->span_f64_n = (int64_t)((d_zero + zo - (uint8_t*)r->span_f64) / 8);
-      if (t == 0) { r->block_sum_off = (int64_t)((uint8_t*)r->span_f64 - d_zero); r->block_dc_off = (int64_t)zo; }
-      for (int a = 0; a < nA; a++) {
-        int op = q->aggregations[a].op;
-        if (op == PB_AGG_DISTINCTCOUNT && !dc_raw[a]) { dt.dc_bits[a] = reinterpret_cast<uint32_t*>(d_zero + zo); dt.dc_words[a] = dc_words[a]; zo += 4 * S * dc_words[a]; }
-        if (op == PB_AGG_DISTINCTCOUNT && dc_raw[a]) { dt.dcnt[a] = reinterpret_cast<unsigned long long*>(d_zero + zo); zo += 8 * S; }
-        if (op == PB_AGG_MIN || op == PB_AGG_MAX) {
-          dt.mm[a] = d_mm + mo; mo += S;
-        }
-      }
-      if (t == 0) { r->span_mm = d_mm; r->span_mm_n = (int64_t)mo; }
-      zo = (zo + 255) & ~(size_t)255;
-      if (table_mode == T_HASH) { dt.hkeys = reinterpret_cast<unsigned long long*>(d_ff + fo); fo += (8 * S * (size_t)key_words + 15) & ~(size_t)15; dt.key_words = key_words; }
-      if (track_first) { dt.first_doc = reinterpret_cast<uint32_t*>(d_ff + fo); fo += (4 * S + 15) & ~(size_t)15; }
-      for (int a = 0; a < nA; a++)
-        if (dc_raw[a]) { dt.dset[a] = reinterpret_cast<unsigned long long*>(d_ff + fo); dt.dset_mask[a] = tm.dset_cap[a] - 1; fo += 16 * tm.dset_cap[a]; }
-      unsigned long long* cnt = r->d_counters + (size_t)t * PB_COUNTERS_PER_TABLE;
-      dt.num_groups = reinterpret_cast<unsigned int*>(cnt + 0);
-      dt.limit_reached = reinterpret_cast<unsigned int*>(cnt + 1);
-      dt.any_limit = reinterpret_cast<unsigned int*>(d_aux + any_limit_off);
-      dt.docs_matched = cnt + 2;
-      dt.num_groups_limit = (uint32_t)std::max(1, q->num_groups_limit);
-      {
-        uint64_t docs = 0;
-        for (int si : tm.seg_idx) docs += (uint64_t)g->segs[si]->num_docs;
-        dt.limit_active = (uint64_t)dt.num_groups_limit < docs ? 1u : 0u;    // groups <= docs: an unreachable limit needs no tickets
-      }
-    }
-    CU(cudaGetLastError());
-  }
+  const size_t seg_stats_bytes = P.nF > 0 ? 8 * (size_t)(1 + PB_MAX_AGG_FILTERS) * (size_t)P.n_segs : 0;   // swim-lane statistics per segment
+  const size_t mm_bytes = (8 * P.mm_elems + 255) & ~(size_t)255;
+  P.any_limit_off = 8 * PB_MAX_WAVES + seg_stats_bytes;   // query-wide "a key was refused" flag (hash tables)
+  const size_t thr_off = P.any_limit_off + 8;              // numGroupsLimit thresholds (one u32 per table), after the statistics
+  P.aux_bytes = (thr_off + (r->track_first ? 4 * (size_t)P.n_tables : 0) + 255) & ~(size_t)255;
+  CU(cudaMallocAsync((void**)&P.d_zero, P.zero_bytes + mm_bytes + P.aux_bytes + 16, st)); r->dev_allocs.push_back(P.d_zero);
+  if (P.ff_bytes) { CU(cudaMallocAsync((void**)&P.d_ff, P.ff_bytes + 16, st)); r->dev_allocs.push_back(P.d_ff); }
+  P.d_aux = P.d_zero + P.zero_bytes + mm_bytes;
+  r->d_first_thr = r->track_first ? reinterpret_cast<uint32_t*>(P.d_aux + thr_off) : nullptr;
+  r->block = P.d_zero; r->block_bytes = (int64_t)(P.zero_bytes + 8 * P.mm_elems);
+  r->block_mm_off = (int64_t)P.zero_bytes;
+  r->d_counters = reinterpret_cast<unsigned long long*>(P.d_zero);
+  r->d_seg_stats = seg_stats_bytes ? reinterpret_cast<unsigned long long*>(P.d_aux + 8 * PB_MAX_WAVES) : nullptr;
+  if ((rc = lay_out_tables(P))) return rc;
+  CU(cudaGetLastError());
 
   if (r->trim_size > 0) {
-    for (int t = 0; t < n_tables; t++) {
-      const uint64_t S = slots_of(r->tables[t]);
+    for (int t = 0; t < P.n_tables; t++) {
+      const uint64_t S = slots_of(P, r->tables[t]);
       unsigned long long* ok = nullptr; DevSelectState* sel = nullptr;
       CU(cudaMallocAsync((void**)&ok, 8 * S, st)); r->dev_allocs.push_back(ok);
       CU(cudaMallocAsync((void**)&sel, sizeof(DevSelectState), st)); r->dev_allocs.push_back(sel);
@@ -2043,15 +2057,19 @@ static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, c
       r->d_okey.push_back(ok); r->d_sel.push_back(sel);
     }
   }
-  lap(1);
-  // ---- query arena (descriptors + leaf payloads) ----
+  return PB_OK;
+}
+
+// The query arena (descriptors + leaf payloads) and the flat bitmaps of the index leaves
+static int alloc_arena(Plan& P) {
+  const int n_segs = P.n_segs, n_tables = P.n_tables;
   size_t arena_cap = (sizeof(DevQuery) + 16) * (1 + PB_MAX_WAVES) + 256 + (sizeof(DevSegQuery) + 64) * (size_t)n_segs + (sizeof(DevTable) + 64) * (size_t)n_tables
-                     + 8 * PB_COUNTERS_PER_TABLE * (size_t)n_tables + 64 + (nF > 0 ? (sizeof(DevLaneWeights) + 16) * (size_t)n_segs : 0)
+                     + 8 * PB_COUNTERS_PER_TABLE * (size_t)n_tables + 64 + (P.nF > 0 ? (sizeof(DevLaneWeights) + 16) * (size_t)n_segs : 0)
                      + (sizeof(DevRowSeg) + 16) * (size_t)n_segs;
   size_t bitmap_words_total = 0;
   for (int si = 0; si < n_segs; si++) {
-    const pb_segment_query& sq = sqs[si];
-    pb_segment_s* s = g->segs[si];
+    const pb_segment_query& sq = P.sqs[si];
+    pb_segment_s* s = P.g->segs[si];
     auto account = [&](const pb_filter_node* nodes, int n_nodes) {
       for (int n = 0; n < n_nodes; n++) {
         const pb_filter_node& fn = nodes[n];
@@ -2068,537 +2086,587 @@ static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, c
       }
     };
     account(sq.filter, sq.num_filter_nodes);
-    for (int f = 0; f < nF; f++) account(sq.agg_filters[f], sq.agg_filter_nodes[f]);
+    for (int f = 0; f < P.nF; f++) account(sq.agg_filters[f], sq.agg_filter_nodes[f]);
   }
-  Arena ar;
+  Arena& ar = P.ar;
   ar.cap = arena_cap; ar.host.resize(arena_cap);
-  CU(cudaMallocAsync((void**)&ar.dev, arena_cap, st)); r->dev_allocs.push_back(ar.dev);
-  uint32_t* d_bitmaps = nullptr;
+  CU(cudaMallocAsync((void**)&ar.dev, arena_cap, P.st)); P.r->dev_allocs.push_back(ar.dev);
   if (bitmap_words_total) {
-    CU(cudaMallocAsync((void**)&d_bitmaps, 4 * bitmap_words_total, st)); r->dev_allocs.push_back(d_bitmaps);
-    CU(cudaMemsetAsync(d_bitmaps, 0, 4 * bitmap_words_total, st));
+    CU(cudaMallocAsync((void**)&P.d_bitmaps, 4 * bitmap_words_total, P.st)); P.r->dev_allocs.push_back(P.d_bitmaps);
+    CU(cudaMemsetAsync(P.d_bitmaps, 0, 4 * bitmap_words_total, P.st));
   }
-
-  DevQuery* hq = nullptr;
-  DevQuery* dq = ar.put<DevQuery>(nullptr, 1, &hq);
-  DevSegQuery* hsegs = nullptr;
-  DevSegQuery* dsegs = ar.put<DevSegQuery>(nullptr, (size_t)n_segs, &hsegs);
+  ar.put<DevQuery>(nullptr, 1, &P.hq);
+  P.d_segs = ar.put<DevSegQuery>(nullptr, (size_t)n_segs, &P.hsegs);
   DevTable* htabs = nullptr;
-  DevTable* dtabs = ar.put<DevTable>(nullptr, (size_t)n_tables, &htabs);
-  for (int t = 0; t < n_tables; t++) htabs[t] = r->tables[t].dev;
+  P.d_tabs = ar.put<DevTable>(nullptr, (size_t)n_tables, &htabs);
+  for (int t = 0; t < n_tables; t++) htabs[t] = P.r->tables[t].dev;
+  P.r->seg_scan_leaves.assign(n_segs, 0);
+  return PB_OK;
+}
 
-  struct PendingExpand { int kind; const uint8_t* inv; int card; const int32_t* ids; int n_ids; uint32_t* out; uint32_t num_docs; std::vector<int32_t> host_ids; };
-  std::vector<PendingExpand> expands;
-  int slot_bits_max[PB_MAX_SCAN_SLOTS] = {0};
-  int set_cache_max = 0;
-  int n_slots_max = 0;
-  bool any_cand_leaf = false;
-  size_t bm_off = 0;
-  r->seg_scan_leaves.assign(n_segs, 0);
+// Where a gathered column is read from: the row-group field `field` (>= 0), else the staged HBM copy, else the caller's
+// mapped host buffer (PB_Q_GATHER_IN_PLACE), which counts towards the result's in_place_columns
+struct GatherSrc { const uint8_t* fwd; uint32_t full_words, tail_word; int32_t stride_bits, bit_off; };
+static GatherSrc gather_source(pb_result_s* r, const Column& c, const RowGroup* rg, int field) {
+  if (!c.fwd_staged) r->in_place_columns++;
+  if (field >= 0) return {rg->d_rows, 0xFFFFFFFFu, 0u, rg->stride_bits, rg->bit_off[(size_t)field]};
+  if (c.fwd_staged) return {c.d_fwd, 0xFFFFFFFFu, 0u, c.has_dict ? c.bits : 8 * c.raw_width, 0};
+  return {c.d_fwd_host, c.host_full_words, c.host_tail_word, c.has_dict ? c.bits : 8 * c.raw_width, 0};
+}
+// the field of dictionary column `col` (form: see RowGroup) in the segment's row group, or -1
+static int rg_field(const RowGroup* rg, const Column& c, int col, int form) { return (rg && c.has_dict) ? rg->find(col, form) : -1; }
 
-  for (int si = 0; si < n_segs; si++) {
-    pb_segment_s* s = g->segs[si];
-    const pb_segment_query& sq = sqs[si];
-    DevSegQuery& ds = hsegs[si];
-    ds.num_docs = s->num_docs;
-    ds.table = combine ? 0 : si;
-    int n_scan = 0, set_smem_used = 0;
-    int slot_of_col[PB_MAX_SCAN_SLOTS];
-    // one postfix filter program -> device nodes + leaves.  force_gather: every scan leaf is tested per doc from its forward
-    // index (FILTER clauses, evaluated by pb_agg_kernel); otherwise the candidate plan decides per leaf.
-    auto build_program = [&](const pb_filter_node* nodes, int n_nodes, int8_t* node_kind, int8_t* node_arg, DevLeaf* leaves, int max_leaves,
-                             int& n_leaves, bool force_gather) -> int {
-    for (int n = 0; n < n_nodes; n++) {
-      const pb_filter_node& fn = nodes[n];
-      if (fn.kind == PB_F_AND || fn.kind == PB_F_OR) {
-        if (fn.num_children < 1 || fn.num_children > PB_MAX_LEAVES) return fail(PB_ERR_UNSUPPORTED, "AND/OR with %d children", fn.num_children);
-        node_kind[n] = fn.kind == PB_F_AND ? N_AND : N_OR; node_arg[n] = (int8_t)fn.num_children; continue;
+struct SegSlots { int n_scan = 0, set_smem_used = 0; int slot_of_col[PB_MAX_SCAN_SLOTS]; };   // scan slots of one segment
+
+// One postfix filter program of segment si -> device nodes + leaves.  force_gather: every scan leaf is tested per doc from its
+// forward index (FILTER clauses, evaluated by the aggregation kernels); otherwise the candidate plan decides per leaf.
+static int lower_program(Plan& P, int si, SegSlots& ss, const pb_filter_node* nodes, int n_nodes, int8_t* node_kind, int8_t* node_arg,
+                         DevLeaf* leaves, int max_leaves, int& n_leaves, bool force_gather) {
+  pb_segment_s* s = P.g->segs[si];
+  pb_result_s* r = P.r;
+  Arena& ar = P.ar;
+  for (int n = 0; n < n_nodes; n++) {
+    const pb_filter_node& fn = nodes[n];
+    if (fn.kind == PB_F_AND || fn.kind == PB_F_OR) {
+      if (fn.num_children < 1 || fn.num_children > PB_MAX_LEAVES) return fail(PB_ERR_UNSUPPORTED, "AND/OR with %d children", fn.num_children);
+      node_kind[n] = fn.kind == PB_F_AND ? N_AND : N_OR; node_arg[n] = (int8_t)fn.num_children; continue;
+    }
+    if (fn.kind == PB_F_NOT) { node_kind[n] = N_NOT; node_arg[n] = 1; continue; }
+    if (n_leaves >= max_leaves) return fail(PB_ERR_UNSUPPORTED, "more than %d filter leaves", max_leaves);
+    DevLeaf& lf = leaves[n_leaves];
+    memset(&lf, 0, sizeof lf);
+    lf.set_smem_off = -1;
+    lf.est_permille = 500;
+    node_kind[n] = N_LEAF; node_arg[n] = (int8_t)n_leaves; n_leaves++;
+    auto scan_slot = [&](const Column& c) -> int {
+      if (force_gather || P.cand_leaf[si][n]) {          // evaluated on candidates: no stage slot, read where the column lies
+        const GatherSrc src = gather_source(r, c, P.seg_rg[si], rg_field(P.seg_rg[si], c, fn.column, 0));
+        lf.gather = 1;
+        lf.gfwd = src.fwd; lf.g_full_words = src.full_words; lf.g_tail_word = src.tail_word;
+        lf.g_stride_bits = src.stride_bits; lf.g_bit_off = src.bit_off;
+        P.any_cand_leaf = true;
+        return PB_MAX_SCAN_SLOTS;      // not a slot index (>= 0 = success)
       }
-      if (fn.kind == PB_F_NOT) { node_kind[n] = N_NOT; node_arg[n] = 1; continue; }
-      if (n_leaves >= max_leaves) return fail(PB_ERR_UNSUPPORTED, "more than %d filter leaves", max_leaves);
-      DevLeaf& lf = leaves[n_leaves];
-      memset(&lf, 0, sizeof lf);
-      lf.set_smem_off = -1;
-      lf.est_permille = 500;
-      node_kind[n] = N_LEAF; node_arg[n] = (int8_t)n_leaves; n_leaves++;
-      auto scan_slot = [&](const Column& c) -> int {
-        if (force_gather || cand_leaf[si][n]) {          // evaluated on candidates: no stage slot, read where the column lies
-          lf.gather = 1;
-          lf.gfwd = c.fwd_staged ? c.d_fwd : c.d_fwd_host;
-          lf.g_full_words = c.fwd_staged ? 0xFFFFFFFFu : c.host_full_words;
-          lf.g_tail_word = c.fwd_staged ? 0u : c.host_tail_word;
-          lf.g_stride_bits = c.bits; lf.g_bit_off = 0;
-          if (!c.has_dict) lf.g_stride_bits = 8 * c.raw_width;
-          if (c.has_dict && seg_rg[si] && seg_rg[si]->find(fn.column, 0) >= 0) {
-            const RowGroup* rg = seg_rg[si];
-            lf.gfwd = rg->d_rows; lf.g_full_words = 0xFFFFFFFFu; lf.g_tail_word = 0u;
-            lf.g_stride_bits = rg->stride_bits; lf.g_bit_off = rg->bit_off[(size_t)rg->find(fn.column, 0)];
-          }
-          if (!c.fwd_staged) r->in_place_columns++;
-          any_cand_leaf = true;
-          return PB_MAX_SCAN_SLOTS;      // not a slot index (>= 0 = success)
+      for (int k = 0; k < ss.n_scan; k++) if (ss.slot_of_col[k] == fn.column) return k;
+      if (ss.n_scan >= PB_MAX_SCAN_SLOTS) return -1;
+      ss.slot_of_col[ss.n_scan] = fn.column;
+      DevScanCol& sc = P.hsegs[si].scan[ss.n_scan];
+      sc.base = c.d_fwd; sc.bits_per_doc = c.has_dict ? c.bits : 8 * c.raw_width; sc.bytes_total = c.d_fwd_bytes;
+      P.slot_bits_max[ss.n_scan] = std::max(P.slot_bits_max[ss.n_scan], sc.bits_per_doc);
+      return ss.n_scan++;
+    };
+    const Column* scanned = nullptr;      // scan leaves: the column they read
+    switch (fn.kind) {
+      case PB_F_MATCH_ALL: lf.kind = L_TRUE; break;
+      case PB_F_EMPTY: lf.kind = L_FALSE; break;
+      case PB_F_SCAN_DICT_RANGE: {
+        const Column& c = s->cols[fn.column];
+        int64_t lo = std::max<int64_t>(fn.lo, 0), hi = std::min<int64_t>(fn.hi, c.card);
+        if (hi <= lo) { lf.kind = L_FALSE; break; }
+        // the whole dictionary: no scan (and span == 2^bits would overflow the top-aligned compare of PredRange::test<W>)
+        if (lo == 0 && hi >= c.card) { lf.kind = L_TRUE; break; }
+        lf.kind = L_DICT_RANGE; lf.bits = c.bits; lf.lo = (uint32_t)lo; lf.span = (uint32_t)(hi - lo);
+        lf.est_permille = (int32_t)(1000.0 * (double)(hi - lo) / (double)c.card);
+        scanned = &c;
+        break;
+      }
+      case PB_F_SCAN_DICT_SET: {
+        const Column& c = s->cols[fn.column];
+        if (fn.num_ids <= 0) { lf.kind = fn.exclusive ? L_TRUE : L_FALSE; break; }
+        size_t words = ((size_t)c.card + 31) / 32;
+        uint32_t* hbits = nullptr;
+        const uint32_t* dbits = ar.put<uint32_t>(nullptr, words, &hbits);
+        if (!dbits) return fail(PB_ERR_STATE, "query arena overflow");
+        for (int k = 0; k < fn.num_ids; k++) {
+          int32_t id = fn.ids[k];
+          if (id < 0 || id >= c.card) return fail(PB_ERR_INVALID, "filter node %d: dictId %d out of range", n, id);
+          hbits[id >> 5] |= 1u << (id & 31);
         }
-        for (int k = 0; k < n_scan; k++) if (slot_of_col[k] == fn.column) return k;
-        if (n_scan >= PB_MAX_SCAN_SLOTS) return -1;
-        slot_of_col[n_scan] = fn.column;
-        DevScanCol& sc = ds.scan[n_scan];
-        sc.base = c.d_fwd; sc.bits_per_doc = c.has_dict ? c.bits : 8 * c.raw_width; sc.bytes_total = c.d_fwd_bytes;
-        slot_bits_max[n_scan] = std::max(slot_bits_max[n_scan], sc.bits_per_doc);
-        return n_scan++;
-      };
-      switch (fn.kind) {
-        case PB_F_MATCH_ALL: lf.kind = L_TRUE; break;
-        case PB_F_EMPTY: lf.kind = L_FALSE; break;
-        case PB_F_SCAN_DICT_RANGE: {
-          const Column& c = s->cols[fn.column];
-          int64_t lo = std::max<int64_t>(fn.lo, 0), hi = std::min<int64_t>(fn.hi, c.card);
-          if (hi <= lo) { lf.kind = L_FALSE; break; }
-          // the whole dictionary: no scan (and span == 2^bits would overflow the top-aligned compare of PredRange::test<W>)
-          if (lo == 0 && hi >= c.card) { lf.kind = L_TRUE; break; }
-          lf.kind = L_DICT_RANGE; lf.bits = c.bits; lf.lo = (uint32_t)lo; lf.span = (uint32_t)(hi - lo);
-          lf.est_permille = (int32_t)(1000.0 * (double)(hi - lo) / (double)c.card);
-          if ((lf.slot = scan_slot(c)) < 0) return fail(PB_ERR_UNSUPPORTED, "more than %d scanned columns", PB_MAX_SCAN_SLOTS);
-          r->seg_scan_leaves[si]++;
-          break;
-        }
-        case PB_F_SCAN_DICT_SET: {
+        lf.kind = L_DICT_SET; lf.bits = c.bits; lf.exclusive = fn.exclusive ? 1 : 0;
+        lf.set_bits = dbits; lf.set_card = c.card;
+        { double f = (double)fn.num_ids / (double)c.card; lf.est_permille = (int32_t)(1000.0 * (fn.exclusive ? 1.0 - f : f)); }
+        if (!force_gather && ss.set_smem_used + c.card <= PB_SET_SMEM_BYTES) { lf.set_smem_off = ss.set_smem_used; ss.set_smem_used += (c.card + 15) & ~15; }
+        scanned = &c;
+        break;
+      }
+      case PB_F_SCAN_RAW_RANGE: {
+        const Column& c = s->cols[fn.column];
+        lf.raw_width = c.raw_width; lf.data_type = c.type;
+        if (c.type == PB_INT || c.type == PB_LONG) { lf.kind = L_RAW_RANGE_I; lf.ilo = fn.lo; lf.ihi = fn.hi; }
+        else { lf.kind = L_RAW_RANGE_F; lf.dlo = fn.dlo; lf.dhi = fn.dhi; lf.dlo_incl = fn.dlo_inclusive; lf.dhi_incl = fn.dhi_inclusive; }
+        scanned = &c;
+        break;
+      }
+      case PB_F_SCAN_RAW_SET: {
+        const Column& c = s->cols[fn.column];
+        if (fn.num_raw_values <= 0) { lf.kind = fn.exclusive ? L_TRUE : L_FALSE; break; }
+        lf.kind = L_RAW_SET; lf.raw_width = c.raw_width; lf.data_type = c.type; lf.exclusive = fn.exclusive ? 1 : 0;
+        lf.raw_set = ar.put<int64_t>(fn.raw_values, (size_t)fn.num_raw_values);
+        lf.n_raw_set = fn.num_raw_values;
+        if (!lf.raw_set) return fail(PB_ERR_STATE, "query arena overflow");
+        scanned = &c;
+        break;
+      }
+      case PB_F_INVERTED: case PB_F_SORTED: case PB_F_BITMAP: {
+        size_t words = (((size_t)s->num_docs + 2047) / 2048) * 64;
+        uint32_t* bm = P.d_bitmaps + P.bm_off; P.bm_off += words;
+        lf.kind = L_BITMAP; lf.bitmap = bm; lf.exclusive = fn.exclusive ? 1 : 0;
+        auto expand_item = [&](int kind) -> DevExpandItem& {
+          P.expand_items.emplace_back();
+          DevExpandItem& it = P.expand_items.back();
+          memset(&it, 0, sizeof it);
+          it.kind = kind; it.out = bm; it.num_docs = (uint32_t)s->num_docs;
+          return it;
+        };
+        if (fn.kind == PB_F_INVERTED) {
           const Column& c = s->cols[fn.column];
           if (fn.num_ids <= 0) { lf.kind = fn.exclusive ? L_TRUE : L_FALSE; break; }
-          size_t words = ((size_t)c.card + 31) / 32;
-          uint32_t* hbits = nullptr;
-          const uint32_t* dbits = ar.put<uint32_t>(nullptr, words, &hbits);
-          if (!dbits) return fail(PB_ERR_STATE, "query arena overflow");
+          for (int k = 0; k < fn.num_ids; k++) if (fn.ids[k] < 0 || fn.ids[k] >= c.card) return fail(PB_ERR_INVALID, "filter node %d: dictId out of range", n);
+          const int32_t* dids = ar.put<int32_t>(fn.ids, (size_t)fn.num_ids);
+          if (!dids) return fail(PB_ERR_STATE, "query arena overflow");
+          for (int k = 0; k < fn.num_ids; k++) { DevExpandItem& it = expand_item(0); it.inv = c.d_inv; it.card = c.card; it.id = fn.ids[k]; }
+        } else if (fn.kind == PB_F_SORTED) {
+          lf.exclusive = 0;
+          if (fn.num_ids <= 0) { lf.kind = L_FALSE; break; }
           for (int k = 0; k < fn.num_ids; k++) {
-            int32_t id = fn.ids[k];
-            if (id < 0 || id >= c.card) return fail(PB_ERR_INVALID, "filter node %d: dictId %d out of range", n, id);
-            hbits[id >> 5] |= 1u << (id & 31);
+            int32_t lo = fn.ids[2 * k], hi = fn.ids[2 * k + 1];
+            if (lo < 0 || hi < lo || hi >= s->num_docs) return fail(PB_ERR_INVALID, "filter node %d: bad docId range [%d,%d]", n, lo, hi);
           }
-          lf.kind = L_DICT_SET; lf.bits = c.bits; lf.exclusive = fn.exclusive ? 1 : 0;
-          lf.set_bits = dbits; lf.set_card = c.card;
-          { double f = (double)fn.num_ids / (double)c.card; lf.est_permille = (int32_t)(1000.0 * (fn.exclusive ? 1.0 - f : f)); }
-          if (!force_gather && set_smem_used + c.card <= PB_SET_SMEM_BYTES) { lf.set_smem_off = set_smem_used; set_smem_used += (c.card + 15) & ~15; }
-          if ((lf.slot = scan_slot(c)) < 0) return fail(PB_ERR_UNSUPPORTED, "more than %d scanned columns", PB_MAX_SCAN_SLOTS);
-          r->seg_scan_leaves[si]++;
-          break;
+          const int32_t* dp = ar.put<int32_t>(fn.ids, 2 * (size_t)fn.num_ids);
+          if (!dp) return fail(PB_ERR_STATE, "query arena overflow");
+          DevExpandItem& it = expand_item(1);
+          it.pairs = dp; it.n_pairs = fn.num_ids;
+        } else {
+          // wrap the caller's Roaring blob as a one-entry inverted index: [BE off0][BE off1][blob]
+          // (no blob: the null-value vector staged with the node's column -- IS NULL / IS NOT NULL, FilterPlanNode.java:294-307)
+          const uint8_t* blob = (const uint8_t*)fn.blob; uint64_t blob_len = fn.blob_len;
+          if (!blob && fn.column >= 0 && fn.column < (int)s->cols.size()) { blob = s->cols[(size_t)fn.column].h_null; blob_len = s->cols[(size_t)fn.column].h_null_len; }
+          if (!blob || blob_len < 8) return fail(PB_ERR_INVALID, "filter node %d: bitmap blob missing (and column %d has no null-value vector)", n, fn.column);
+          std::vector<uint8_t> tmp(8 + blob_len);
+          uint32_t o0 = 8, o1 = (uint32_t)(8 + blob_len);
+          tmp[0] = o0 >> 24; tmp[1] = o0 >> 16; tmp[2] = o0 >> 8; tmp[3] = (uint8_t)o0;
+          tmp[4] = o1 >> 24; tmp[5] = o1 >> 16; tmp[6] = o1 >> 8; tmp[7] = (uint8_t)o1;
+          memcpy(tmp.data() + 8, blob, blob_len);
+          const uint8_t* dblob = ar.put<uint8_t>(tmp.data(), tmp.size());
+          static const int32_t zero_id = 0;
+          const int32_t* dids = ar.put<int32_t>(&zero_id, 1);
+          if (!dblob || !dids) return fail(PB_ERR_STATE, "query arena overflow");
+          DevExpandItem& it = expand_item(0);
+          it.inv = dblob; it.card = 1; it.id = 0;
         }
-        case PB_F_SCAN_RAW_RANGE: {
-          const Column& c = s->cols[fn.column];
-          lf.raw_width = c.raw_width; lf.data_type = c.type;
-          if (c.type == PB_INT || c.type == PB_LONG) { lf.kind = L_RAW_RANGE_I; lf.ilo = fn.lo; lf.ihi = fn.hi; }
-          else { lf.kind = L_RAW_RANGE_F; lf.dlo = fn.dlo; lf.dhi = fn.dhi; lf.dlo_incl = fn.dlo_inclusive; lf.dhi_incl = fn.dhi_inclusive; }
-          if ((lf.slot = scan_slot(c)) < 0) return fail(PB_ERR_UNSUPPORTED, "more than %d scanned columns", PB_MAX_SCAN_SLOTS);
-          r->seg_scan_leaves[si]++;
-          break;
-        }
-        case PB_F_SCAN_RAW_SET: {
-          const Column& c = s->cols[fn.column];
-          if (fn.num_raw_values <= 0) { lf.kind = fn.exclusive ? L_TRUE : L_FALSE; break; }
-          lf.kind = L_RAW_SET; lf.raw_width = c.raw_width; lf.data_type = c.type; lf.exclusive = fn.exclusive ? 1 : 0;
-          lf.raw_set = ar.put<int64_t>(fn.raw_values, (size_t)fn.num_raw_values);
-          lf.n_raw_set = fn.num_raw_values;
-          if (!lf.raw_set) return fail(PB_ERR_STATE, "query arena overflow");
-          if ((lf.slot = scan_slot(c)) < 0) return fail(PB_ERR_UNSUPPORTED, "more than %d scanned columns", PB_MAX_SCAN_SLOTS);
-          r->seg_scan_leaves[si]++;
-          break;
-        }
-        case PB_F_INVERTED: case PB_F_SORTED: case PB_F_BITMAP: {
-          size_t words = (((size_t)s->num_docs + 2047) / 2048) * 64;
-          uint32_t* bm = d_bitmaps + bm_off; bm_off += words;
-          lf.kind = L_BITMAP; lf.bitmap = bm; lf.exclusive = fn.exclusive ? 1 : 0;
-          if (fn.kind == PB_F_INVERTED) {
-            const Column& c = s->cols[fn.column];
-            if (fn.num_ids <= 0) { lf.kind = fn.exclusive ? L_TRUE : L_FALSE; break; }
-            for (int k = 0; k < fn.num_ids; k++) if (fn.ids[k] < 0 || fn.ids[k] >= c.card) return fail(PB_ERR_INVALID, "filter node %d: dictId out of range", n);
-            const int32_t* dids = ar.put<int32_t>(fn.ids, (size_t)fn.num_ids);
-            if (!dids) return fail(PB_ERR_STATE, "query arena overflow");
-            expands.push_back({0, c.d_inv, c.card, dids, fn.num_ids, bm, (uint32_t)s->num_docs, std::vector<int32_t>(fn.ids, fn.ids + fn.num_ids)});
-          } else if (fn.kind == PB_F_SORTED) {
-            lf.exclusive = 0;
-            if (fn.num_ids <= 0) { lf.kind = L_FALSE; break; }
-            for (int k = 0; k < fn.num_ids; k++) {
-              int32_t lo = fn.ids[2 * k], hi = fn.ids[2 * k + 1];
-              if (lo < 0 || hi < lo || hi >= s->num_docs) return fail(PB_ERR_INVALID, "filter node %d: bad docId range [%d,%d]", n, lo, hi);
-            }
-            const int32_t* dp = ar.put<int32_t>(fn.ids, 2 * (size_t)fn.num_ids);
-            if (!dp) return fail(PB_ERR_STATE, "query arena overflow");
-            expands.push_back({1, nullptr, 0, dp, fn.num_ids, bm, (uint32_t)s->num_docs, {}});
-          } else {
-            // wrap the caller's Roaring blob as a one-entry inverted index: [BE off0][BE off1][blob]
-            // (no blob: the null-value vector staged with the node's column -- IS NULL / IS NOT NULL, FilterPlanNode.java:294-307)
-            const uint8_t* blob = (const uint8_t*)fn.blob; uint64_t blob_len = fn.blob_len;
-            if (!blob && fn.column >= 0 && fn.column < (int)s->cols.size()) { blob = s->cols[(size_t)fn.column].h_null; blob_len = s->cols[(size_t)fn.column].h_null_len; }
-            if (!blob || blob_len < 8) return fail(PB_ERR_INVALID, "filter node %d: bitmap blob missing (and column %d has no null-value vector)", n, fn.column);
-            std::vector<uint8_t> tmp(8 + blob_len);
-            uint32_t o0 = 8, o1 = (uint32_t)(8 + blob_len);
-            tmp[0] = o0 >> 24; tmp[1] = o0 >> 16; tmp[2] = o0 >> 8; tmp[3] = (uint8_t)o0;
-            tmp[4] = o1 >> 24; tmp[5] = o1 >> 16; tmp[6] = o1 >> 8; tmp[7] = (uint8_t)o1;
-            memcpy(tmp.data() + 8, blob, blob_len);
-            const uint8_t* dblob = ar.put<uint8_t>(tmp.data(), tmp.size());
-            static const int32_t zero_id = 0;
-            const int32_t* dids = ar.put<int32_t>(&zero_id, 1);
-            if (!dblob || !dids) return fail(PB_ERR_STATE, "query arena overflow");
-            expands.push_back({0, dblob, 1, dids, 1, bm, (uint32_t)s->num_docs, std::vector<int32_t>(1, 0)});
-          }
-          break;
-        }
-        default: return fail(PB_ERR_INVALID, "filter node %d: unknown kind %d", n, fn.kind);
+        break;
       }
-      if (lf.gather) lf.slot = -1;
+      default: return fail(PB_ERR_INVALID, "filter node %d: unknown kind %d", n, fn.kind);
     }
-    return PB_OK;
-    };
-    ds.n_nodes = sq.num_filter_nodes;
-    {
-      int nl = 0;
-      if ((rc = build_program(sq.filter, sq.num_filter_nodes, ds.node_kind, ds.node_arg, ds.leaves, PB_MAX_LEAVES, nl, false))) return rc;
+    if (scanned) {
+      if ((lf.slot = scan_slot(*scanned)) < 0) return fail(PB_ERR_UNSUPPORTED, "more than %d scanned columns", PB_MAX_SCAN_SLOTS);
+      r->seg_scan_leaves[si]++;
     }
-    // FILTER(WHERE ...) clauses
-    ds.n_agg_filters = nF;
-    {
-      int nl = 0, nn = 0;
-      for (int f = 0; f < nF; f++) {
-        ds.af_begin[f] = nn;
-        if (nn + sq.agg_filter_nodes[f] > PB_MAX_AF_NODES) return fail(PB_ERR_UNSUPPORTED, "FILTER clauses have more than %d nodes", PB_MAX_AF_NODES);
-        if ((rc = build_program(sq.agg_filters[f], sq.agg_filter_nodes[f], ds.af_node_kind + nn, ds.af_node_arg + nn, ds.af_leaves, PB_MAX_AF_LEAVES, nl, true))) return rc;
-        nn += sq.agg_filter_nodes[f];
-      }
-      for (int f = nF; f <= PB_MAX_AGG_FILTERS; f++) ds.af_begin[f] = nn;
-      ds.af_docs = d_seg_stats ? d_seg_stats + (size_t)si * (1 + PB_MAX_AGG_FILTERS) : nullptr;
-    }
-    ds.n_scan = n_scan;
-    set_cache_max = std::max(set_cache_max, set_smem_used);
-    n_slots_max = std::max(n_slots_max, n_scan);
-    r->n_scan_leaves_total += (int)r->seg_scan_leaves[si];
+    if (lf.gather) lf.slot = -1;
+  }
+  return PB_OK;
+}
 
-    // group-by / aggregation columns
-    const TableMeta& tm = r->tables[ds.table];
-    uint64_t mult = 1;
+// DevSegQuery of segment si: its filter program, its FILTER clauses, and where its key and aggregation columns are read
+static int bind_segment(Plan& P, int si) {
+  int rc;
+  pb_segment_s* s = P.g->segs[si];
+  const pb_segment_query& sq = P.sqs[si];
+  const pb_query_desc* q = P.q;
+  const int nG = P.nG, nF = P.nF;
+  DevSegQuery& ds = P.hsegs[si];
+  ds.num_docs = s->num_docs;
+  ds.table = P.combine ? 0 : si;
+  SegSlots ss;
+  ds.n_nodes = sq.num_filter_nodes;
+  {
+    int nl = 0;
+    if ((rc = lower_program(P, si, ss, sq.filter, sq.num_filter_nodes, ds.node_kind, ds.node_arg, ds.leaves, PB_MAX_LEAVES, nl, false))) return rc;
+  }
+  // FILTER(WHERE ...) clauses
+  ds.n_agg_filters = nF;
+  {
+    int nl = 0, nn = 0;
+    for (int f = 0; f < nF; f++) {
+      ds.af_begin[f] = nn;
+      if (nn + sq.agg_filter_nodes[f] > PB_MAX_AF_NODES) return fail(PB_ERR_UNSUPPORTED, "FILTER clauses have more than %d nodes", PB_MAX_AF_NODES);
+      if ((rc = lower_program(P, si, ss, sq.agg_filters[f], sq.agg_filter_nodes[f], ds.af_node_kind + nn, ds.af_node_arg + nn, ds.af_leaves, PB_MAX_AF_LEAVES, nl, true))) return rc;
+      nn += sq.agg_filter_nodes[f];
+    }
+    for (int f = nF; f <= PB_MAX_AGG_FILTERS; f++) ds.af_begin[f] = nn;
+    ds.af_docs = P.r->d_seg_stats ? P.r->d_seg_stats + (size_t)si * (1 + PB_MAX_AGG_FILTERS) : nullptr;
+  }
+  ds.n_scan = ss.n_scan;
+  P.set_cache_max = std::max(P.set_cache_max, ss.set_smem_used);
+  P.n_slots_max = std::max(P.n_slots_max, ss.n_scan);
+
+  // group-by / aggregation columns
+  const TableMeta& tm = P.r->tables[ds.table];
+  const RowGroup* rg = P.seg_rg[si];
+  uint64_t mult = 1;
+  for (int j = 0; j < nG; j++) {
+    const Column& c = s->cols[P.gcol[si][j]];
+    DevKeyCol& kc = ds.keys[j];
+    const GatherSrc src = gather_source(P.r, c, rg, rg_field(rg, c, P.gcol[si][j], 0));
+    kc.fwd = src.fwd; kc.n_full_words = src.full_words; kc.tail_word = src.tail_word;
+    kc.bits = c.bits; kc.raw_width = c.has_dict ? 0 : c.raw_width; kc.data_type = c.type;
+    kc.stride_bits = src.stride_bits; kc.bit_off = src.bit_off;
+    kc.remap = (P.combine && P.gdict[j]) ? P.gdict[j]->d_remap[si] : nullptr;
+    kc.shift = tm.shifts[j];
+    kc.mult = mult;
+    if (tm.cards[j] > 0) mult *= (uint64_t)tm.cards[j];
+    if (!c.has_dict && (c.type == PB_FLOAT) && nG > 1) return fail(PB_ERR_UNSUPPORTED, "raw FLOAT key in a multi-column group-by");
+  }
+  for (int a = 0; a < P.nA; a++) {
+    const int ci = P.acol[si][a];
+    if (ci < 0) continue;
+    const Column& c = s->cols[ci];
+    DevAggCol& ac = ds.aggs[a];
+    // a numeric input may be a decoded value field of the row group: read like a raw column, no dictionary lookup
+    const int fv = q->aggregations[a].op != PB_AGG_DISTINCTCOUNT ? rg_field(rg, c, ci, 1) : -1;
+    const GatherSrc src = gather_source(P.r, c, rg, fv >= 0 ? fv : rg_field(rg, c, ci, 0));
+    ac.fwd = src.fwd; ac.n_full_words = src.full_words; ac.tail_word = src.tail_word;
+    ac.dict_f64 = c.d_dict_f64; ac.bits = c.bits; ac.raw_width = fv >= 0 ? c.entry_bytes : c.has_dict ? 0 : c.raw_width; ac.data_type = c.type;
+    ac.stride_bits = src.stride_bits; ac.bit_off = src.bit_off;
+    ac.remap = (P.combine && P.adict[a]) ? P.adict[a]->d_remap[si] : nullptr;
+  }
+  return PB_OK;
+}
+
+// Plan-time specialisation of the aggregation (pb_agg_rows_kernel): a dense table, every key a dictionary column and every
+// aggregation COUNT(*) or a numeric column, all of them fields of row groups of one stride
+static int plan_rows_kernel(Plan& P) {
+  static const bool rows_on = []() { const char* e = getenv("PB_AGG_ROWS"); return !e || atoi(e) != 0; }();
+  const pb_query_desc* q = P.q;
+  const int n_segs = P.n_segs, nG = P.nG, nA = P.nA;
+  int rw = 0;
+  bool ok = rows_on && P.r->table_mode == T_DENSE && P.nF == 0 && nG > 0 && n_segs > 0;
+  for (int si = 0; si < n_segs && ok; si++) {
+    const RowGroup* rg = P.seg_rg[si];
+    if (!rg || (rw && rw != rg->stride_bits / 32)) { ok = false; break; }
+    rw = rg->stride_bits / 32;
+    for (int j = 0; j < nG && ok; j++) if (rg->find(P.gcol[si][j], 0) < 0) ok = false;
+    for (int a = 0; a < nA && ok; a++) {
+      const int op = q->aggregations[a].op;
+      if (op == PB_AGG_COUNT) continue;
+      if (op == PB_AGG_DISTINCTCOUNT || rg->find(P.acol[si][a], 1) < 0) ok = false;
+    }
+  }
+  if (!ok) return PB_OK;
+  P.rows_rw = rw;
+  P.d_row_segs = P.ar.put<DevRowSeg>(nullptr, (size_t)n_segs, &P.h_row_segs);
+  if (!P.d_row_segs) return fail(PB_ERR_STATE, "query arena overflow");
+  for (int si = 0; si < n_segs; si++) {
+    // every key and aggregation input is a row-group field: bind_segment already read them from there
+    const DevSegQuery& ds = P.hsegs[si];
+    DevRowSeg& rs = P.h_row_segs[si];
+    rs.rows = reinterpret_cast<const uint32_t*>(P.seg_rg[si]->d_rows);
+    rs.table = ds.table;
     for (int j = 0; j < nG; j++) {
-      const Column& c = s->cols[gcol[si][j]];
-      DevKeyCol& kc = ds.keys[j];
-      kc.fwd = c.fwd_staged ? c.d_fwd : c.d_fwd_host; kc.n_full_words = c.fwd_staged ? 0xFFFFFFFFu : c.host_full_words;
-      kc.tail_word = c.fwd_staged ? 0u : c.host_tail_word; if (!c.fwd_staged) r->in_place_columns++;
-      kc.bits = c.bits; kc.raw_width = c.has_dict ? 0 : c.raw_width; kc.data_type = c.type;
-      kc.stride_bits = c.has_dict ? c.bits : 8 * c.raw_width; kc.bit_off = 0;
-      if (c.has_dict && seg_rg[si] && seg_rg[si]->find(gcol[si][j], 0) >= 0) {
-        const RowGroup* rg = seg_rg[si];
-        kc.fwd = rg->d_rows; kc.n_full_words = 0xFFFFFFFFu; kc.tail_word = 0u;
-        kc.stride_bits = rg->stride_bits; kc.bit_off = rg->bit_off[(size_t)rg->find(gcol[si][j], 0)];
-      }
-      kc.remap = (combine && gdict[j]) ? gdict[j]->d_remap[si] : nullptr;
-      kc.shift = tm.shifts[j];
-      kc.mult = mult;
-      if (tm.cards[j] > 0) mult *= (uint64_t)tm.cards[j];
-      if (!c.has_dict && (c.type == PB_FLOAT) && nG > 1) return fail(PB_ERR_UNSUPPORTED, "raw FLOAT key in a multi-column group-by");
+      const DevKeyCol& kc = ds.keys[j];
+      rs.keys[j].off = (uint32_t)kc.bit_off; rs.keys[j].bits = (uint32_t)kc.bits; rs.keys[j].mult = kc.mult; rs.keys[j].remap = kc.remap;
     }
     for (int a = 0; a < nA; a++) {
-      if (acol[si][a] < 0) continue;
-      const Column& c = s->cols[acol[si][a]];
-      DevAggCol& ac = ds.aggs[a];
-      ac.fwd = c.fwd_staged ? c.d_fwd : c.d_fwd_host; ac.n_full_words = c.fwd_staged ? 0xFFFFFFFFu : c.host_full_words;
-      ac.tail_word = c.fwd_staged ? 0u : c.host_tail_word; if (!c.fwd_staged) r->in_place_columns++;
-      ac.dict_f64 = c.d_dict_f64; ac.bits = c.bits; ac.raw_width = c.has_dict ? 0 : c.raw_width; ac.data_type = c.type;
-      ac.stride_bits = c.has_dict ? c.bits : 8 * c.raw_width; ac.bit_off = 0;
-      if (c.has_dict && seg_rg[si]) {
-        const RowGroup* rg = seg_rg[si];
-        const int fv = q->aggregations[a].op != PB_AGG_DISTINCTCOUNT ? rg->find(acol[si][a], 1) : -1, fi = rg->find(acol[si][a], 0);
-        if (fv >= 0) {            // decoded value field: read like a raw column, no dictionary lookup
-          ac.fwd = rg->d_rows; ac.n_full_words = 0xFFFFFFFFu; ac.tail_word = 0u;
-          ac.raw_width = c.entry_bytes; ac.stride_bits = rg->stride_bits; ac.bit_off = rg->bit_off[(size_t)fv];
-        } else if (fi >= 0) {
-          ac.fwd = rg->d_rows; ac.n_full_words = 0xFFFFFFFFu; ac.tail_word = 0u;
-          ac.stride_bits = rg->stride_bits; ac.bit_off = rg->bit_off[(size_t)fi];
-        }
-      }
-      ac.remap = (combine && adict[a]) ? adict[a]->d_remap[si] : nullptr;
+      if (q->aggregations[a].op == PB_AGG_COUNT) continue;
+      const DevAggCol& ac = ds.aggs[a];
+      rs.aggs[a].off = (uint32_t)ac.bit_off; rs.aggs[a].width = (uint32_t)ac.raw_width; rs.aggs[a].type = (uint32_t)ac.data_type; rs.aggs[a].exact_int = 0;
     }
   }
-
-  // ---- plan-time specialisation of the aggregation (pb_agg_rows_kernel): a dense table, every key a dictionary column
-  // and every aggregation COUNT(*) or a numeric column, all of them fields of row groups of one stride ----
-  const DevRowSeg* d_row_segs = nullptr;
-  int rows_rw = 0;
-  {
-    static const bool rows_on = []() { const char* e = getenv("PB_AGG_ROWS"); return !e || atoi(e) != 0; }();
-    bool ok = rows_on && table_mode == T_DENSE && nF == 0 && nG > 0 && n_segs > 0;
-    for (int si = 0; si < n_segs && ok; si++) {
-      const RowGroup* rg = seg_rg[si];
-      if (!rg || (rows_rw && rows_rw != rg->stride_bits / 32)) { ok = false; break; }
-      rows_rw = rg->stride_bits / 32;
-      for (int j = 0; j < nG && ok; j++) if (rg->find(gcol[si][j], 0) < 0) ok = false;
-      for (int a = 0; a < nA && ok; a++) {
-        const int op = q->aggregations[a].op;
-        if (op == PB_AGG_COUNT) continue;
-        if (op == PB_AGG_DISTINCTCOUNT || rg->find(acol[si][a], 1) < 0) ok = false;
-      }
-    }
-    if (ok) {
-      DevRowSeg* h_rs = nullptr;
-      d_row_segs = ar.put<DevRowSeg>(nullptr, (size_t)n_segs, &h_rs);
-      if (!d_row_segs) return fail(PB_ERR_STATE, "query arena overflow");
-      for (int si = 0; si < n_segs; si++) {
-        const RowGroup* rg = seg_rg[si];
-        const pb_segment_s* sg = g->segs[si];
-        DevRowSeg& rs = h_rs[si];
-        rs.rows = reinterpret_cast<const uint32_t*>(rg->d_rows);
-        rs.table = hsegs[si].table;
-        for (int j = 0; j < nG; j++) {
-          const DevKeyCol& kc = hsegs[si].keys[j];
-          rs.keys[j].off = (uint32_t)rg->bit_off[(size_t)rg->find(gcol[si][j], 0)];
-          rs.keys[j].bits = (uint32_t)sg->cols[gcol[si][j]].bits;
-          rs.keys[j].mult = kc.mult; rs.keys[j].remap = kc.remap;
-        }
-        for (int a = 0; a < nA; a++) {
-          if (q->aggregations[a].op == PB_AGG_COUNT) continue;
-          const Column& c = sg->cols[acol[si][a]];
-          rs.aggs[a].off = (uint32_t)rg->bit_off[(size_t)rg->find(acol[si][a], 1)];
-          rs.aggs[a].width = (uint32_t)c.entry_bytes; rs.aggs[a].type = (uint32_t)c.type; rs.aggs[a].exact_int = 0;
-        }
-      }
-      // SUM / AVG over INT / LONG columns: when max|value| x docs < 2^53 every partial sum is an integer a double holds
-      // exactly, so the CTA-private table may accumulate them as 64-bit integers with two native 32-bit shared-memory
-      // atomics instead of a compare-and-swap loop on a double -- bit-identical to the reference's double accumulation,
-      // whatever the order (DevRowAgg::exact_int)
-      static const bool exact_on = []() { const char* e = getenv("PB_AGG_EXACT_INT"); return !e || atoi(e) != 0; }();
-      uint64_t docs_all = 0;
-      for (int si = 0; si < n_segs; si++) docs_all += (uint64_t)g->segs[si]->num_docs;
-      for (int a = 0; a < nA && exact_on; a++) {
-        const int op = q->aggregations[a].op;
-        if (op != PB_AGG_SUM && op != PB_AGG_AVG) continue;
-        bool exact = true;
-        for (int si = 0; si < n_segs && exact; si++) {
-          const Column& c = g->segs[si]->cols[acol[si][a]];
-          if (!c.has_dict || c.card <= 0 || (c.type != PB_INT && c.type != PB_LONG) || c.h_dict.size() < (size_t)c.card * (size_t)c.entry_bytes) { exact = false; break; }
-          // sorted dictionary: the extremes are its first and last entries
-          const uint8_t* lo = c.h_dict.data(); const uint8_t* hi = c.h_dict.data() + (size_t)(c.card - 1) * (size_t)c.entry_bytes;
-          const int64_t vlo = c.type == PB_INT ? (int64_t)(int32_t)be32(lo) : (int64_t)be64(lo);
-          const int64_t vhi = c.type == PB_INT ? (int64_t)(int32_t)be32(hi) : (int64_t)be64(hi);
-          const uint64_t alo = vlo < 0 ? (uint64_t)0 - (uint64_t)vlo : (uint64_t)vlo, ahi = vhi < 0 ? (uint64_t)0 - (uint64_t)vhi : (uint64_t)vhi;
-          const uint64_t bound = std::max<uint64_t>(std::max(alo, ahi), 1);
-          if (bound >= (1ull << 53) || docs_all >= (1ull << 53) / bound) exact = false;
-        }
-        if (exact) for (int si = 0; si < n_segs; si++) h_rs[si].aggs[a].exact_int = 1;
-      }
-    } else rows_rw = 0;
-  }
-
-  // ---- work-unit geometry: one stage = one unit (U x 1024 docs) of every scan slot, per warp ----
-  int sum_bits = 0;
-  for (int k = 0; k < n_slots_max; k++) sum_bits += slot_bits_max[k];
-  static const int unit_env = []() { const char* e = getenv("PB_UNIT"); return e ? atoi(e) : 2; }();
-  auto stage_bytes_for = [&](int U, int32_t* offs) {
-    size_t b = 0;
-    for (int k = 0; k < n_slots_max; k++) {
-      if (offs) offs[k] = (int32_t)b;
-      b += (((size_t)U * PB_CHUNK_DOCS * slot_bits_max[k] / 8 + 16) + 15) & ~(size_t)15;
-    }
-    return b;
-  };
-  // two chunks per unit halve the per-unit overhead (dispatch, TMA issue, list append) when two CTAs still fit an SM
-  int U = (unit_env == 1) ? 1 : 2;
-  if (U == 2 && stage_bytes_for(2, nullptr) * PB_NSTAGE * PB_NWARPS > 100 * 1024) U = 1;
-  int32_t slot_offs[PB_MAX_SCAN_SLOTS] = {0};
-  size_t stage_bytes = stage_bytes_for(U, slot_offs);
-  if (stage_bytes * PB_NSTAGE * PB_NWARPS > 200 * 1024)
-    return fail(PB_ERR_UNSUPPORTED, "scan predicates touch %d bits per row: unit stages do not fit shared memory", sum_bits);
-  const uint64_t unit_docs = (uint64_t)U * PB_CHUNK_DOCS;
-  uint64_t n_chunks = 0, n_docs_total = 0;
-  bool match_all = true;
-  for (int si = 0; si < n_segs; si++) {
-    hsegs[si].unit_begin = n_chunks;
-    hsegs[si].n_units = ((uint64_t)g->segs[si]->num_docs + unit_docs - 1) / unit_docs;
-    hsegs[si].doc_base = n_docs_total;
-    n_chunks += hsegs[si].n_units;
-    n_docs_total += (uint64_t)g->segs[si]->num_docs;
-    if (sqs[si].num_filter_nodes != 0) match_all = false;
-  }
-  if (d_row_segs) {
-    DevRowSeg* h_rs = reinterpret_cast<DevRowSeg*>(ar.host.data() + (reinterpret_cast<const uint8_t*>(d_row_segs) - ar.dev));
-    for (int si = 0; si < n_segs; si++) h_rs[si].doc_base = hsegs[si].doc_base;
-  }
-  if (n_docs_total >= (1ull << 32)) return fail(PB_ERR_UNSUPPORTED, "%llu docs in one call (match list is 32-bit): split the segment group", (unsigned long long)n_docs_total);
-  // ---- how the matches reach the group table (see pb_device.cuh):
-  //   smem      one dense table that fits shared memory and enough matches to amortise merging one private copy per CTA
-  //   global    everything else: pb_agg_kernel, one thread per match, reductions straight into the global table
-  // (a third way -- the filter kernel aggregating its own matches, no match list -- was measured and removed: the two
-  //  kernels are bound by the same memory system and did not overlap)
-  const bool fuse = false;
-  int n_acc = 0, n_fc = 0;
-  for (int a = 0; a < nA; a++) {
+  // SUM / AVG over INT / LONG columns: when max|value| x docs < 2^53 every partial sum is an integer a double holds
+  // exactly, so the CTA-private table may accumulate them as 64-bit integers with two native 32-bit shared-memory
+  // atomics instead of a compare-and-swap loop on a double -- bit-identical to the reference's double accumulation,
+  // whatever the order (DevRowAgg::exact_int)
+  static const bool exact_on = []() { const char* e = getenv("PB_AGG_EXACT_INT"); return !e || atoi(e) != 0; }();
+  uint64_t docs_all = 0;
+  for (int si = 0; si < n_segs; si++) docs_all += (uint64_t)P.g->segs[si]->num_docs;
+  for (int a = 0; a < nA && exact_on; a++) {
     const int op = q->aggregations[a].op;
+    if (op != PB_AGG_SUM && op != PB_AGG_AVG) continue;
+    bool exact = true;
+    for (int si = 0; si < n_segs && exact; si++) {
+      const Column& c = P.g->segs[si]->cols[P.acol[si][a]];
+      if (!c.has_dict || c.card <= 0 || (c.type != PB_INT && c.type != PB_LONG) || c.h_dict.size() < (size_t)c.card * (size_t)c.entry_bytes) { exact = false; break; }
+      // sorted dictionary: the extremes are its first and last entries
+      const uint8_t* lo = c.h_dict.data(); const uint8_t* hi = c.h_dict.data() + (size_t)(c.card - 1) * (size_t)c.entry_bytes;
+      const int64_t vlo = c.type == PB_INT ? (int64_t)(int32_t)be32(lo) : (int64_t)be64(lo);
+      const int64_t vhi = c.type == PB_INT ? (int64_t)(int32_t)be32(hi) : (int64_t)be64(hi);
+      const uint64_t alo = vlo < 0 ? (uint64_t)0 - (uint64_t)vlo : (uint64_t)vlo, ahi = vhi < 0 ? (uint64_t)0 - (uint64_t)vhi : (uint64_t)vhi;
+      const uint64_t bound = std::max<uint64_t>(std::max(alo, ahi), 1);
+      if (bound >= (1ull << 53) || docs_all >= (1ull << 53) / bound) exact = false;
+    }
+    if (exact) for (int si = 0; si < n_segs; si++) P.h_row_segs[si].aggs[a].exact_int = 1;
+  }
+  return PB_OK;
+}
+
+// Work-unit geometry: one stage = one unit (U x 1024 docs) of every scan slot, per warp
+static size_t stage_bytes_for(const Plan& P, int U, int32_t* offs) {
+  size_t b = 0;
+  for (int k = 0; k < P.n_slots_max; k++) {
+    if (offs) offs[k] = (int32_t)b;
+    b += (((size_t)U * PB_CHUNK_DOCS * P.slot_bits_max[k] / 8 + 16) + 15) & ~(size_t)15;
+  }
+  return b;
+}
+static int plan_units(Plan& P) {
+  int sum_bits = 0;
+  for (int k = 0; k < P.n_slots_max; k++) sum_bits += P.slot_bits_max[k];
+  static const int unit_env = []() { const char* e = getenv("PB_UNIT"); return e ? atoi(e) : 2; }();
+  // two chunks per unit halve the per-unit overhead (dispatch, TMA issue, list append) when two CTAs still fit an SM
+  P.U = (unit_env == 1) ? 1 : 2;
+  if (P.U == 2 && stage_bytes_for(P, 2, nullptr) * PB_NSTAGE * PB_NWARPS > 100 * 1024) P.U = 1;
+  P.stage_bytes = stage_bytes_for(P, P.U, P.hq->slot_off);
+  if (P.stage_bytes * PB_NSTAGE * PB_NWARPS > 200 * 1024)
+    return fail(PB_ERR_UNSUPPORTED, "scan predicates touch %d bits per row: unit stages do not fit shared memory", sum_bits);
+  const uint64_t unit_docs = (uint64_t)P.U * PB_CHUNK_DOCS;
+  for (int si = 0; si < P.n_segs; si++) {
+    DevSegQuery& ds = P.hsegs[si];
+    ds.unit_begin = P.n_chunks;
+    ds.n_units = ((uint64_t)P.g->segs[si]->num_docs + unit_docs - 1) / unit_docs;
+    ds.doc_base = P.n_docs_total;
+    if (P.h_row_segs) P.h_row_segs[si].doc_base = ds.doc_base;
+    P.n_chunks += ds.n_units;
+    P.n_docs_total += (uint64_t)P.g->segs[si]->num_docs;
+    if (P.sqs[si].num_filter_nodes != 0) P.match_all = false;
+  }
+  if (P.n_docs_total >= (1ull << 32)) return fail(PB_ERR_UNSUPPORTED, "%llu docs in one call (match list is 32-bit): split the segment group", (unsigned long long)P.n_docs_total);
+  return PB_OK;
+}
+
+// How the matches reach the group table (see pb_device.cuh):
+//   smem      one dense table that fits shared memory and enough matches to amortise merging one private copy per CTA
+//   global    everything else: pb_agg_kernel, one thread per match, reductions straight into the global table
+// (rows: pb_agg_rows_kernel, see plan_rows_kernel).  A third way -- the filter kernel aggregating its own matches, no
+// match list -- was measured and removed: the two kernels are bound by the same memory system and did not overlap.
+static int plan_match_path(Plan& P) {
+  pb_result_s* r = P.r;
+  int n_acc = 0, n_fc = 0;
+  for (int a = 0; a < P.nA; a++) {
+    const int op = P.q->aggregations[a].op;
     if (op >= PB_AGG_SUM && op <= PB_AGG_AVG) n_acc++;
-    if (nF > 0 && q->agg_filter_of[a] >= 0 && (op == PB_AGG_COUNT || op == PB_AGG_AVG || count_all)) n_fc++;
+    if (has_fcnt(P.q, a)) n_fc++;
   }
   static const int smem_table_env = []() { const char* e = getenv("PB_AGG_SMEM"); return e ? atoi(e) : 1; }();
   static const size_t smem_table_budget = 200 * 1024;
-  size_t st_rep_bytes = 0; int st_replicas = 0;
-  if (smem_table_env && !fuse && !track_first && table_mode == T_DENSE && n_tables == 1 && r->tables[0].capacity <= (1u << 20)) {
-    st_rep_bytes = pb_smem_table_bytes((uint32_t)r->tables[0].capacity, n_fc, n_acc);
-    if (st_rep_bytes <= smem_table_budget) { st_replicas = 1; while (st_replicas < 32 && (size_t)(2 * st_replicas) * st_rep_bytes <= smem_table_budget) st_replicas *= 2; }
+  if (smem_table_env && !r->track_first && r->table_mode == T_DENSE && P.n_tables == 1 && r->tables[0].capacity <= (1u << 20)) {
+    P.st_rep_bytes = pb_smem_table_bytes((uint32_t)r->tables[0].capacity, n_fc, n_acc);
+    if (P.st_rep_bytes <= smem_table_budget) { P.st_replicas = 1; while (P.st_replicas < 32 && (size_t)(2 * P.st_replicas) * P.st_rep_bytes <= smem_table_budget) P.st_replicas *= 2; }
   }
-  const bool use_smem_table = st_replicas > 0;
-  uint32_t* d_match_list = nullptr;
-  if (!match_all && !fuse && n_docs_total > 0) {
-    r->scratch = scratch_alloc(ctx, 4 * (size_t)n_docs_total + 256, &r->scratch_cap);
-    if (!r->scratch) return fail(PB_ERR_OOM, "match list allocation (%zu bytes) failed", 4 * (size_t)n_docs_total + 256);
-    d_match_list = (uint32_t*)r->scratch;
+  if (!P.match_all && P.n_docs_total > 0) {
+    r->scratch = scratch_alloc(P.ctx, 4 * (size_t)P.n_docs_total + 256, &r->scratch_cap);
+    if (!r->scratch) return fail(PB_ERR_OOM, "match list allocation (%zu bytes) failed", 4 * (size_t)P.n_docs_total + 256);
+    P.d_match_list = (uint32_t*)r->scratch;
   }
-  r->match_all = match_all;
-  r->n_agg_filters = nF; r->count_all = count_all;
-  // ---- counter cells that the host knows up front (ExecutionStatistics; see PB_COUNTERS_PER_TABLE) ----
+  return PB_OK;
+}
+
+// Counter cells that the host knows up front (ExecutionStatistics; see PB_COUNTERS_PER_TABLE), and the layout fingerprint
+static int fill_counters_head(Plan& P) {
+  pb_result_s* r = P.r;
+  const pb_query_desc* q = P.q;
   unsigned long long* h_head = nullptr;
-  const unsigned long long* d_head = ar.put<unsigned long long>(nullptr, (size_t)PB_COUNTERS_PER_TABLE * n_tables, &h_head);
-  if (!d_head) return fail(PB_ERR_STATE, "query arena overflow");
-  for (int si = 0; si < n_segs; si++) {
-    unsigned long long* c = h_head + (size_t)hsegs[si].table * PB_COUNTERS_PER_TABLE;
-    const unsigned long long nd = (unsigned long long)g->segs[si]->num_docs;
-    if (match_all) c[2] += nd;                                   // numDocsScanned of a match-all query (no filter kernel)
+  P.d_head = P.ar.put<unsigned long long>(nullptr, (size_t)PB_COUNTERS_PER_TABLE * P.n_tables, &h_head);
+  if (!P.d_head) return fail(PB_ERR_STATE, "query arena overflow");
+  for (int si = 0; si < P.n_segs; si++) {
+    unsigned long long* c = h_head + (size_t)P.hsegs[si].table * PB_COUNTERS_PER_TABLE;
+    const unsigned long long nd = (unsigned long long)P.g->segs[si]->num_docs;
+    if (P.match_all) c[2] += nd;                                 // numDocsScanned of a match-all query (no filter kernel)
     c[6] += nd;                                                  // numTotalDocs
     c[7] += (unsigned long long)r->seg_scan_leaves[si] * nd;     // every scan leaf reads every doc of the segment on the device
     c[8] += 1;
   }
-  {
-    // what must agree across ranks for the blocks to be mergeable element by element
-    unsigned long long fp = 0xcbf29ce484222325ull;
-    auto mix = [&](unsigned long long v) { fp ^= v; fp *= 0x100000001b3ull; fp ^= fp >> 29; };
-    mix((unsigned long long)r->block_bytes); mix((unsigned long long)r->block_sum_off); mix((unsigned long long)r->block_dc_off); mix((unsigned long long)r->block_mm_off);
-    mix((unsigned long long)table_mode); mix((unsigned long long)nG); mix((unsigned long long)nA); mix((unsigned long long)nF);
-    for (int a = 0; a < nA; a++) mix((unsigned long long)q->aggregations[a].op * 131 + dc_words[a]);
-    for (auto& tm : r->tables) { mix(tm.capacity); for (auto cd : tm.cards) mix((unsigned long long)cd); }
-    r->fingerprint = fp >> 8;                               // head room: n_ranks x fp must not wrap
-    for (int t = 0; t < n_tables; t++) h_head[(size_t)t * PB_COUNTERS_PER_TABLE + 9] = r->fingerprint;
-  }
-  // ---- filtered aggregations: which swim-lanes exist per segment, and how many columns each projects
-  // (AggregationFunctionUtils.buildFilteredAggregationInfos :312-400; statistics are summed lane by lane,
-  // FilteredGroupByOperator.java:146-149): one lane per FILTER clause over (main AND clause) -- unless the clause matches all
-  // under a real main filter, then its functions join the non-filtered lane -- plus the non-filtered lane when it has
-  // functions or the query groups; an empty main filter is a single lane without docs ----
-  const DevLaneWeights* d_lane_w = nullptr;
-  if (nF > 0) {
-    r->agg_filter_of.assign(q->agg_filter_of, q->agg_filter_of + nA);
-    auto classify = [](const pb_filter_node* nodes, int n) { return n == 0 ? 1 : (n == 1 && nodes[0].kind == PB_F_MATCH_ALL ? 1 : (n == 1 && nodes[0].kind == PB_F_EMPTY ? 2 : 0)); };
-    auto lane_cols = [&](const std::vector<char>& in_lane) {
-      std::vector<std::string> cols;
-      for (auto& nme : r->gb_names) if (std::find(cols.begin(), cols.end(), nme) == cols.end()) cols.push_back(nme);
-      for (int a = 0; a < nA; a++) if (in_lane[a] && !r->agg_cols[a].empty() && std::find(cols.begin(), cols.end(), r->agg_cols[a]) == cols.end()) cols.push_back(r->agg_cols[a]);
-      return (int32_t)cols.size();
-    };
-    DevLaneWeights* h_lw = nullptr;
-    d_lane_w = ar.put<DevLaneWeights>(nullptr, (size_t)n_segs, &h_lw);
-    if (!d_lane_w) return fail(PB_ERR_STATE, "query arena overflow");
-    for (int si = 0; si < n_segs; si++) {
-      DevLaneWeights& lw = h_lw[si];
-      lw.table = hsegs[si].table;
-      const int main_kind = classify(sqs[si].filter, sqs[si].num_filter_nodes);
-      if (main_kind == 2) continue;                        // empty main filter: no docs in any lane
-      std::vector<char> in_main(nA, 0);
-      bool any_main = false;
-      for (int f = 0; f < nF; f++) {
-        std::vector<char> in_lane(nA, 0);
-        for (int a = 0; a < nA; a++) if (q->agg_filter_of[a] == f) in_lane[a] = 1;
-        if (main_kind != 1 && classify(sqs[si].agg_filters[f], sqs[si].agg_filter_nodes[f]) == 1) {
-          for (int a = 0; a < nA; a++) if (in_lane[a]) { in_main[a] = 1; any_main = true; }
-          continue;
-        }
-        lw.docs_w[1 + f] = 1; lw.post_w[1 + f] = lane_cols(in_lane);
-      }
-      for (int a = 0; a < nA; a++) if (q->agg_filter_of[a] < 0) { in_main[a] = 1; any_main = true; }
-      if (any_main || nG > 0) { lw.docs_w[0] = 1; lw.post_w[0] = lane_cols(in_main); }
-    }
-  }
+  // what must agree across ranks for the blocks to be mergeable element by element
+  unsigned long long fp = 0xcbf29ce484222325ull;
+  auto mix = [&](unsigned long long v) { fp ^= v; fp *= 0x100000001b3ull; fp ^= fp >> 29; };
+  mix((unsigned long long)r->block_bytes); mix((unsigned long long)r->block_sum_off); mix((unsigned long long)r->block_dc_off); mix((unsigned long long)r->block_mm_off);
+  mix((unsigned long long)r->table_mode); mix((unsigned long long)P.nG); mix((unsigned long long)P.nA); mix((unsigned long long)P.nF);
+  for (int a = 0; a < P.nA; a++) mix((unsigned long long)q->aggregations[a].op * 131 + P.dc_words[a]);
+  for (auto& tm : r->tables) { mix(tm.capacity); for (auto cd : tm.cards) mix((unsigned long long)cd); }
+  r->fingerprint = fp >> 8;                               // head room: n_ranks x fp must not wrap
+  for (int t = 0; t < P.n_tables; t++) h_head[(size_t)t * PB_COUNTERS_PER_TABLE + 9] = r->fingerprint;
+  return PB_OK;
+}
 
-  hq->n_segs = n_segs; hq->n_group_by = nG; hq->n_aggs = nA; hq->table_mode = table_mode;
-  for (int a = 0; a < nA; a++) hq->agg_op[a] = q->aggregations[a].op;
-  for (int a = 0; a < PB_MAX_AGGS; a++) hq->agg_filter_of[a] = (nF > 0 && a < nA) ? q->agg_filter_of[a] : -1;
-  hq->n_agg_filters = nF;
-  for (int k = 0; k < n_slots_max; k++) hq->slot_off[k] = slot_offs[k];
-  hq->stage_bytes = (int32_t)stage_bytes;
-  hq->set_cache_bytes = set_cache_max;
+// Filtered aggregations: which swim-lanes exist per segment, and how many columns each projects
+// (AggregationFunctionUtils.buildFilteredAggregationInfos :312-400; statistics are summed lane by lane,
+// FilteredGroupByOperator.java:146-149): one lane per FILTER clause over (main AND clause) -- unless the clause matches all
+// under a real main filter, then its functions join the non-filtered lane -- plus the non-filtered lane when it has
+// functions or the query groups; an empty main filter is a single lane without docs
+static int plan_lane_weights(Plan& P) {
+  if (P.nF == 0) return PB_OK;
+  pb_result_s* r = P.r;
+  const pb_query_desc* q = P.q;
+  const int nA = P.nA;
+  auto classify = [](const pb_filter_node* nodes, int n) { return n == 0 ? 1 : (n == 1 && nodes[0].kind == PB_F_MATCH_ALL ? 1 : (n == 1 && nodes[0].kind == PB_F_EMPTY ? 2 : 0)); };
+  auto lane_cols = [&](const std::vector<char>& in_lane) {
+    std::vector<std::string> cols;
+    for (auto& nme : r->gb_names) if (std::find(cols.begin(), cols.end(), nme) == cols.end()) cols.push_back(nme);
+    for (int a = 0; a < nA; a++) if (in_lane[a] && !r->agg_cols[a].empty() && std::find(cols.begin(), cols.end(), r->agg_cols[a]) == cols.end()) cols.push_back(r->agg_cols[a]);
+    return (int32_t)cols.size();
+  };
+  DevLaneWeights* h_lw = nullptr;
+  P.d_lane_w = P.ar.put<DevLaneWeights>(nullptr, (size_t)P.n_segs, &h_lw);
+  if (!P.d_lane_w) return fail(PB_ERR_STATE, "query arena overflow");
+  for (int si = 0; si < P.n_segs; si++) {
+    DevLaneWeights& lw = h_lw[si];
+    lw.table = P.hsegs[si].table;
+    const int main_kind = classify(P.sqs[si].filter, P.sqs[si].num_filter_nodes);
+    if (main_kind == 2) continue;                        // empty main filter: no docs in any lane
+    std::vector<char> in_main(nA, 0);
+    bool any_main = false;
+    for (int f = 0; f < P.nF; f++) {
+      std::vector<char> in_lane(nA, 0);
+      for (int a = 0; a < nA; a++) if (q->agg_filter_of[a] == f) in_lane[a] = 1;
+      if (main_kind != 1 && classify(P.sqs[si].agg_filters[f], P.sqs[si].agg_filter_nodes[f]) == 1) {
+        for (int a = 0; a < nA; a++) if (in_lane[a]) { in_main[a] = 1; any_main = true; }
+        continue;
+      }
+      lw.docs_w[1 + f] = 1; lw.post_w[1 + f] = lane_cols(in_lane);
+    }
+    for (int a = 0; a < nA; a++) if (q->agg_filter_of[a] < 0) { in_main[a] = 1; any_main = true; }
+    if (any_main || P.nG > 0) { lw.docs_w[0] = 1; lw.post_w[0] = lane_cols(in_main); }
+  }
+  return PB_OK;
+}
+
+// The launch-wide DevQuery
+static void fill_query(Plan& P) {
+  const pb_query_desc* q = P.q;
+  pb_result_s* r = P.r;
+  DevQuery* hq = P.hq;
+  hq->n_segs = P.n_segs; hq->n_group_by = P.nG; hq->n_aggs = P.nA; hq->table_mode = r->table_mode;
+  for (int a = 0; a < P.nA; a++) hq->agg_op[a] = q->aggregations[a].op;
+  for (int a = 0; a < PB_MAX_AGGS; a++) hq->agg_filter_of[a] = (P.nF > 0 && a < P.nA) ? q->agg_filter_of[a] : -1;
+  hq->n_agg_filters = P.nF;
+  hq->stage_bytes = (int32_t)P.stage_bytes;
+  hq->set_cache_bytes = P.set_cache_max;
   hq->out_cap = PB_OUT_CAP; hq->cand_cap = PB_CAND_CAP;
-  hq->cand_bytes = any_cand_leaf ? (int32_t)(2 * PB_CAND_CAP * PB_NWARPS) : 0;   // u16 offsets inside the unit, one list per warp
+  hq->cand_bytes = P.any_cand_leaf ? (int32_t)(2 * PB_CAND_CAP * PB_NWARPS) : 0;   // u16 offsets inside the unit, one list per warp
   hq->use_tma = (q->flags & PB_Q_NO_TMA) ? 0 : 1;
   hq->generic = (q->flags & PB_Q_GENERIC_KERNEL) ? 1 : 0;
-  hq->n_units = n_chunks; hq->segs = dsegs; hq->tables = dtabs;
-  hq->n_docs_total = n_docs_total; hq->match_all = match_all ? 1 : 0;
+  hq->n_units = P.n_chunks; hq->segs = P.d_segs; hq->tables = P.d_tabs;
+  hq->n_docs_total = P.n_docs_total; hq->match_all = P.match_all ? 1 : 0;
   { static const int sm = []() { const char* e = getenv("PB_SPARSE_MAX"); return e ? atoi(e) : PB_SPARSE_MAX; }(); hq->sparse_max = sm; }
-  hq->match_list = d_match_list;
-  if (use_smem_table) {
-    hq->st_slots = (int32_t)r->tables[0].capacity; hq->st_replicas = st_replicas;
+  hq->match_list = P.d_match_list;
+  if (P.st_replicas > 0) {
+    hq->st_slots = (int32_t)r->tables[0].capacity; hq->st_replicas = P.st_replicas;
     // merging a CTA's private table costs up to one RED per slot and aggregate: it pays once a CTA sees several matches per slot
     static const long long min_env = []() { const char* e = getenv("PB_AGG_SMEM_MIN"); return e ? atoll(e) : -1ll; }();
-    hq->st_min_docs = min_env >= 0 ? (uint64_t)min_env : 4ull * (uint64_t)ctx->num_sms * r->tables[0].capacity;
+    hq->st_min_docs = min_env >= 0 ? (uint64_t)min_env : 4ull * (uint64_t)P.ctx->num_sms * r->tables[0].capacity;
   }
-  r->fused = fuse; r->smem_table = use_smem_table;
-  hq->match_count = reinterpret_cast<unsigned long long*>(d_aux);   // PB_MAX_WAVES zeroed cells (aux region)
-  hq->any_limit = reinterpret_cast<const unsigned int*>(d_aux + any_limit_off);
+  hq->match_count = reinterpret_cast<unsigned long long*>(P.d_aux);   // PB_MAX_WAVES zeroed cells (aux region)
+  hq->any_limit = reinterpret_cast<const unsigned int*>(P.d_aux + P.any_limit_off);
   r->repair_pass = false;
-  if (table_mode == T_HASH) for (auto& tm : r->tables) if (tm.dev.limit_active) r->repair_pass = true;
+  if (r->table_mode == T_HASH) for (auto& tm : r->tables) if (tm.dev.limit_active) r->repair_pass = true;
+}
 
-  // expand items (one per inverted-index bitmap / per sorted-index range list)
-  int n_expand_items = 0;
-  for (auto& e : expands) n_expand_items += e.kind == 0 ? e.n_ids : 1;
-  const DevExpandItem* d_expand_items = nullptr;
-  if (n_expand_items > 0) {
-    std::vector<DevExpandItem> items;
-    items.reserve((size_t)n_expand_items);
-    for (auto& e : expands) {
-      if (e.kind == 0) {
-        for (int k = 0; k < e.n_ids; k++) {
-          DevExpandItem it; memset(&it, 0, sizeof it);
-          it.inv = e.inv; it.out = e.out; it.kind = 0; it.card = e.card; it.id = e.host_ids[k]; it.num_docs = e.num_docs;
-          items.push_back(it);
-        }
-      } else {
-        DevExpandItem it; memset(&it, 0, sizeof it);
-        it.pairs = e.ids; it.out = e.out; it.kind = 1; it.n_pairs = e.n_ids; it.num_docs = e.num_docs;
-        items.push_back(it);
-      }
-    }
-    d_expand_items = ar.put<DevExpandItem>(items.data(), items.size());
-    if (!d_expand_items) return fail(PB_ERR_STATE, "query arena overflow");
-  }
-  // ---- waves: when some segments are still being copied to HBM, launch per run of segments so that the kernels of
-  // one wave (and its in-place gathers over PCIe) overlap the staging copies of the next ----
-  struct Wave { int seg_lo, seg_hi; DevQuery dq; uint64_t n_units, n_docs; };   // the descriptor travels as a __grid_constant__ kernel parameter
-  std::vector<Wave> waves;
-  if (n_pending > 0 && !match_all && n_expand_items == 0 && n_segs > 1 && n_chunks > 0) {
+static int put_expand_items(Plan& P) {
+  if (P.expand_items.empty()) return PB_OK;
+  P.d_expand_items = P.ar.put<DevExpandItem>(P.expand_items.data(), P.expand_items.size());
+  if (!P.d_expand_items) return fail(PB_ERR_STATE, "query arena overflow");
+  return PB_OK;
+}
+
+// Waves: when some segments are still being copied to HBM, launch per run of segments so that the kernels of one wave (and
+// its in-place gathers over PCIe) overlap the staging copies of the next.  Each wave's DevQuery travels as a
+// __grid_constant__ kernel parameter.
+static int plan_waves(Plan& P) {
+  std::vector<pb_result_s::WaveLaunch>& waves = P.r->rp.waves;
+  const int n_segs = P.n_segs;
+  if (P.n_pending > 0 && !P.match_all && P.expand_items.empty() && n_segs > 1 && P.n_chunks > 0) {
     const int per_wave = (n_segs + PB_MAX_WAVES - 1) / PB_MAX_WAVES;
     for (int lo = 0; lo < n_segs; lo += per_wave) {
       const int hi = std::min(n_segs, lo + per_wave);
-      DevQuery w = *hq;
-      w.unit_lo = hsegs[lo].unit_begin;
-      w.n_units = hsegs[hi - 1].unit_begin + hsegs[hi - 1].n_units - w.unit_lo;
-      w.n_docs_total = hsegs[hi - 1].doc_base + (uint64_t)g->segs[hi - 1]->num_docs - hsegs[lo].doc_base;
-      w.match_list = d_match_list + hsegs[lo].doc_base;
-      w.match_count = hq->match_count + waves.size();
-      waves.push_back({lo, hi, w, w.n_units, w.n_docs_total});
+      pb_result_s::WaveLaunch w;
+      w.seg_lo = lo; w.seg_hi = hi;
+      w.dq = *P.hq;
+      w.dq.unit_lo = P.hsegs[lo].unit_begin;
+      w.dq.n_units = P.hsegs[hi - 1].unit_begin + P.hsegs[hi - 1].n_units - w.dq.unit_lo;
+      w.dq.n_docs_total = P.hsegs[hi - 1].doc_base + (uint64_t)P.g->segs[hi - 1]->num_docs - P.hsegs[lo].doc_base;
+      w.dq.match_list = P.d_match_list + P.hsegs[lo].doc_base;
+      w.dq.match_count = P.hq->match_count + waves.size();
+      w.n_units = w.dq.n_units; w.n_docs = w.dq.n_docs_total;
+      waves.push_back(w);
     }
   } else {
-    for (int si = 0; si < n_segs; si++) if (seg_wait[si]) CU(cudaStreamWaitEvent(st, seg_wait[si], 0));
-    waves.push_back({0, n_segs, *hq, n_chunks, n_docs_total});
+    for (int si = 0; si < n_segs; si++) if (P.seg_wait[si]) CU(cudaStreamWaitEvent(P.st, P.seg_wait[si], 0));
+    pb_result_s::WaveLaunch w;
+    w.dq = *P.hq; w.seg_lo = 0; w.seg_hi = n_segs; w.n_units = P.n_chunks; w.n_docs = P.n_docs_total;
+    waves.push_back(w);
   }
-  r->waves = (int)waves.size();
-  CU(cudaMemcpyAsync(ar.dev, ar.host.data(), ar.used, cudaMemcpyHostToDevice, st));
-  {
-    // table init: all regions are 16-byte multiples (cudaMallocAsync alignment is 256)
-    const uint64_t zn = (zero_bytes + 15) / 16, fn = (ff_bytes + 15) / 16, mn = (8 * mm_elems + 15) / 16, an = (aux_bytes + 15) / 16;
-    const uint64_t mx = std::max(std::max(zn, an), std::max(fn, mn));
-    int grid = (int)std::min<uint64_t>((mx + 255) / 256, (uint64_t)ctx->num_sms * 8);
-    if (grid < 1) grid = 1;
-    r->init = {(uint4*)d_zero, zn, (uint4*)d_ff, fn, (uint4*)d_mm, mn, (uint4*)d_aux, an, reinterpret_cast<const uint4*>(d_head),
-               (uint64_t)PB_COUNTERS_PER_TABLE * n_tables / 2, grid};
-    r->key_words = key_words;
-  }
-  lap(2);
+  return PB_OK;
+}
 
-  // ---- launch geometry of the two hot kernels ----
+// Upload the arena and record the arguments of the table init kernel
+static int upload_descriptors(Plan& P) {
+  pb_result_s* r = P.r;
+  CU(cudaMemcpyAsync(P.ar.dev, P.ar.host.data(), P.ar.used, cudaMemcpyHostToDevice, P.st));
+  // table init: all regions are 16-byte multiples (cudaMallocAsync alignment is 256)
+  const uint64_t zn = (P.zero_bytes + 15) / 16, fn = (P.ff_bytes + 15) / 16, mn = (8 * P.mm_elems + 15) / 16, an = (P.aux_bytes + 15) / 16;
+  const uint64_t mx = std::max(std::max(zn, an), std::max(fn, mn));
+  int grid = (int)std::min<uint64_t>((mx + 255) / 256, (uint64_t)P.ctx->num_sms * 8);
+  if (grid < 1) grid = 1;
+  long long* d_mm = P.mm_elems ? reinterpret_cast<long long*>(P.d_zero + P.zero_bytes) : nullptr;
+  r->init = {(uint4*)P.d_zero, zn, (uint4*)P.d_ff, fn, (uint4*)d_mm, mn, (uint4*)P.d_aux, an, reinterpret_cast<const uint4*>(P.d_head),
+             (uint64_t)PB_COUNTERS_PER_TABLE * P.n_tables / 2, grid};
+  return PB_OK;
+}
+
+// Dynamic shared memory of the filter kernel
+static size_t filter_smem(const Plan& P, int out_cap, int cand_cap) {
+  return ((sizeof(FilterSmemHeader) + 127) & ~(size_t)127) + (((size_t)P.set_cache_max + 127) & ~(size_t)127) + (P.any_cand_leaf ? (size_t)2 * cand_cap * PB_NWARPS : 0) +
+         (size_t)PB_NWARPS * out_cap * 4 + P.stage_bytes * PB_NSTAGE * PB_NWARPS;
+}
+
+// Plan-time specialisation: every segment of the launch is "one streamed dictionary leaf of the same width and predicate
+// kind + candidate leaves" -> the small kernel compiled for exactly that (pb_filter_spec.cu).  On success it takes over the
+// filter launch: rp.spec_w / spec_pk, its shared memory and CTAs per launch.
+static void plan_filter_spec(Plan& P, size_t& smem, uint64_t& max_ctas) {
+  static const bool spec_on = []() { const char* e = getenv("PB_FILTER_SPEC"); return !e || atoi(e) != 0; }();
+  pb_result_s::Replay& rp = P.r->rp;
+  if (!(spec_on && !P.match_all && P.n_chunks > 0 && rp.U == 2 && rp.u2_three && !P.hq->generic && P.hq->use_tma)) return;
+  int w = -1, pk = -1;
+  for (int si = 0; si < P.n_segs; si++) {
+    const DevSegQuery& ds = P.hsegs[si];
+    int nl = 0, dense = -1, n_dense = 0;
+    for (int n = 0; n < ds.n_nodes; n++) {
+      if (ds.node_kind[n] == N_LEAF) {
+        const DevLeaf& lf = ds.leaves[ds.node_arg[n]];
+        if (!lf.gather) { dense = ds.node_arg[n]; n_dense++; }
+        nl++;
+      } else if (!(ds.node_kind[n] == N_AND && n == ds.n_nodes - 1 && ds.node_arg[n] == nl)) return;
+    }
+    if (n_dense != 1) return;
+    const DevLeaf& lf = ds.leaves[dense];
+    const int k = lf.kind == L_DICT_RANGE ? 0 : (lf.kind == L_DICT_SET && lf.set_smem_off >= 0) ? 1 : -1;
+    if (k < 0 || (w >= 0 && (w != lf.bits || pk != k))) return;
+    w = lf.bits; pk = k;
+  }
+  if (w <= 0 || !pb_filter_spec_available(w, pk)) return;
+  // the specialised kernel needs 64 registers: a fourth CTA fits an SM when its shared memory does -- halve the
+  // per-warp output buffer and candidate list for that (more flushes / candidate passes, both cheap)
+  size_t smem_spec = smem;
+  int oc = PB_OUT_CAP, cc = PB_CAND_CAP;
+  if (4 * (filter_smem(P, PB_OUT_CAP / 2, PB_CAND_CAP / 2) + 1024) <= 227 * 1024 && 4 * (smem + 1024) > 227 * 1024) { oc /= 2; cc /= 2; smem_spec = filter_smem(P, oc, cc); }
+  int occ = 0;
+  if (pb_filter_spec_prepare(w, pk, smem_spec, &occ) == cudaSuccess && occ >= 1) {
+    rp.spec_w = w; rp.spec_pk = pk; max_ctas = (uint64_t)P.ctx->num_sms * (uint64_t)occ; smem = smem_spec;
+    P.hq->out_cap = oc; P.hq->cand_cap = cc; P.hq->cand_bytes = P.any_cand_leaf ? (int32_t)(2 * cc * PB_NWARPS) : 0;
+    for (auto& wv : rp.waves) { wv.dq.out_cap = oc; wv.dq.cand_cap = cc; wv.dq.cand_bytes = P.hq->cand_bytes; }
+  } else cudaGetLastError();
+}
+
+// Kernel choice and launch geometry of the call, saved in r->rp so that a cached plan can enqueue them again
+static int plan_launches(Plan& P) {
+  Context* ctx = P.ctx;
+  pb_result_s* r = P.r;
+  pb_result_s::Replay& rp = r->rp;
   {
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (!ctx->smem_attr_set) {
       CU(cudaFuncSetAttribute(pb_filter_kernel<1, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       CU(cudaFuncSetAttribute(pb_filter_kernel<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       CU(cudaFuncSetAttribute(pb_filter_kernel<2, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      CU(cudaFuncSetAttribute(pb_agg_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
       CU(cudaFuncSetAttribute(pb_agg_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
       CU(cudaFuncSetAttribute(pb_agg_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 16 * 1024));
       CU(cudaFuncSetAttribute(pb_agg_rows_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 32 * 1024));
@@ -2607,105 +2675,109 @@ static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, c
       ctx->smem_attr_set = true;
     }
   }
-  auto filter_smem = [&](int out_cap, int cand_cap) {
-    return ((sizeof(FilterSmemHeader) + 127) & ~(size_t)127) + (((size_t)set_cache_max + 127) & ~(size_t)127) + (any_cand_leaf ? (size_t)2 * cand_cap * PB_NWARPS : 0) +
-           (size_t)PB_NWARPS * out_cap * 4 + stage_bytes * PB_NSTAGE * PB_NWARPS;
-  };
+  rp.U = P.U;
   size_t smem = 0;
   uint64_t max_ctas = 0;
-  bool u2_three = false;
-  if (!match_all && n_chunks > 0) {
-    smem = filter_smem(PB_OUT_CAP, PB_CAND_CAP);
+  if (!P.match_all && P.n_chunks > 0) {
+    smem = filter_smem(P, PB_OUT_CAP, PB_CAND_CAP);
     if (smem > 227 * 1024) return fail(PB_ERR_UNSUPPORTED, "filter kernel needs %zu bytes of shared memory", smem);
     int occ = 1;
     // U = 2 comes in two register budgets: 3 CTAs/SM (80 registers) when three stages sets fit shared memory, else 2 CTAs/SM
-    u2_three = U == 2 && 3 * (smem + 1024) <= 227 * 1024;
-    if (U == 1) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb_filter_kernel<1, 3>, PB_NTHREADS, smem));
-    else if (u2_three) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb_filter_kernel<2, 3>, PB_NTHREADS, smem));
+    rp.u2_three = P.U == 2 && 3 * (smem + 1024) <= 227 * 1024;
+    if (P.U == 1) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb_filter_kernel<1, 3>, PB_NTHREADS, smem));
+    else if (rp.u2_three) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb_filter_kernel<2, 3>, PB_NTHREADS, smem));
     else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb_filter_kernel<2, 2>, PB_NTHREADS, smem));
     if (occ < 1) return fail(PB_ERR_CUDA, "filter kernel does not fit an SM (smem %zu)", smem);
     max_ctas = (uint64_t)ctx->num_sms * (uint64_t)occ;
   }
-  // ---- plan-time specialisation: every segment of the launch is "one streamed dictionary leaf of the same width and
-  // predicate kind + candidate leaves" -> the small kernel compiled for exactly that (pb_filter_spec.cu) ----
-  int spec_w = 0, spec_pk = 0;
-  {
-    static const bool spec_on = []() { const char* e = getenv("PB_FILTER_SPEC"); return !e || atoi(e) != 0; }();
-    if (spec_on && !match_all && n_chunks > 0 && U == 2 && u2_three && !hq->generic && hq->use_tma) {
-      int w = -1, pk = -1;
-      bool ok = true;
-      for (int si = 0; si < n_segs && ok; si++) {
-        const DevSegQuery& ds = hsegs[si];
-        int nl = 0, dense = -1, n_dense = 0;
-        for (int n = 0; n < ds.n_nodes && ok; n++) {
-          if (ds.node_kind[n] == N_LEAF) {
-            const DevLeaf& lf = ds.leaves[ds.node_arg[n]];
-            if (!lf.gather) { dense = ds.node_arg[n]; n_dense++; }
-            nl++;
-          } else if (!(ds.node_kind[n] == N_AND && n == ds.n_nodes - 1 && ds.node_arg[n] == nl)) ok = false;
-        }
-        if (!ok || n_dense != 1) { ok = false; break; }
-        const DevLeaf& lf = ds.leaves[dense];
-        const int k = lf.kind == L_DICT_RANGE ? 0 : (lf.kind == L_DICT_SET && lf.set_smem_off >= 0) ? 1 : -1;
-        if (k < 0 || (w >= 0 && (w != lf.bits || pk != k))) { ok = false; break; }
-        w = lf.bits; pk = k;
-      }
-      if (ok && w > 0 && pb_filter_spec_available(w, pk)) {
-        // the specialised kernel needs 64 registers: a fourth CTA fits an SM when its shared memory does -- halve the
-        // per-warp output buffer and candidate list for that (more flushes / candidate passes, both cheap)
-        size_t smem_spec = smem;
-        int oc = PB_OUT_CAP, cc = PB_CAND_CAP;
-        if (4 * (filter_smem(PB_OUT_CAP / 2, PB_CAND_CAP / 2) + 1024) <= 227 * 1024 && 4 * (smem + 1024) > 227 * 1024) { oc /= 2; cc /= 2; smem_spec = filter_smem(oc, cc); }
-        int occ = 0;
-        if (pb_filter_spec_prepare(w, pk, smem_spec, &occ) == cudaSuccess && occ >= 1) {
-          spec_w = w; spec_pk = pk; max_ctas = (uint64_t)ctx->num_sms * (uint64_t)occ; smem = smem_spec;
-          hq->out_cap = oc; hq->cand_cap = cc; hq->cand_bytes = any_cand_leaf ? (int32_t)(2 * cc * PB_NWARPS) : 0;
-          for (auto& wv : waves) { wv.dq.out_cap = oc; wv.dq.cand_cap = cc; wv.dq.cand_bytes = hq->cand_bytes; }
-        } else cudaGetLastError();
-      }
-    }
-  }
-  const size_t smem2 = table_mode == T_KEYLESS ? (nF > 0 ? 3 : 2) * sizeof(double) * (size_t)nA * PB_NTHREADS : 0;
+  plan_filter_spec(P, smem, max_ctas);
+  rp.smem_filter = smem;
+  const bool use_smem_table = P.st_replicas > 0;
+  const size_t smem2 = r->table_mode == T_KEYLESS ? (P.nF > 0 ? 3 : 2) * sizeof(double) * (size_t)P.nA * PB_NTHREADS : 0;
   // more resident threads = more gathers in flight (the kernel is DRAM-latency bound); 6 CTAs/SM costs a 4-byte spill
-  static const int agg_occ = []() { const char* e = getenv("PB_AGG_OCC"); int v = e ? atoi(e) : 6; return v == 4 ? 4 : 6; }();
   uint64_t max2 = 0;
-  if (n_docs_total > 0 && !fuse && !use_smem_table) {
+  if (P.n_docs_total > 0 && !use_smem_table) {
     int occ2 = 1;
-    if (agg_occ == 4) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ2, pb_agg_kernel<4>, PB_NTHREADS, smem2));
-    else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ2, pb_agg_kernel<6>, PB_NTHREADS, smem2));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ2, pb_agg_kernel<6>, PB_NTHREADS, smem2));
     if (occ2 < 1) return fail(PB_ERR_CUDA, "aggregation kernel does not fit an SM");
     max2 = (uint64_t)ctx->num_sms * (uint64_t)occ2;
   }
-  {
-    pb_result_s::Replay& rp = r->rp;
-    rp.expand_items = d_expand_items; rp.n_expand = n_expand_items;
-    rp.U = U; rp.u2_three = u2_three; rp.smem_filter = smem; rp.spec_w = spec_w; rp.spec_pk = spec_pk;
-    rp.agg_kind = (fuse || n_docs_total == 0) ? 0 : d_row_segs ? 4 : use_smem_table ? 3 : agg_occ == 4 ? 2 : 1;
-    rp.smem_agg = (use_smem_table && rp.agg_kind >= 3) ? (size_t)st_replicas * st_rep_bytes : rp.agg_kind == 4 ? 0 : smem2;
-    rp.row_segs = d_row_segs; rp.rows_rw = rows_rw;
-    rp.lane_w = d_lane_w; rp.n_lanes = 1 + nF; rp.n_segs = n_segs;
-    rp.flags = q->flags;
-    for (const Wave& w : waves) {
-      pb_result_s::WaveLaunch wl;
-      wl.dq = w.dq; wl.seg_lo = w.seg_lo; wl.seg_hi = w.seg_hi; wl.n_units = w.n_units; wl.n_docs = w.n_docs;
-      // every CTA gets a contiguous range of chunks; keep at least one chunk per warp
-      wl.grid_filter = (!match_all && w.n_units > 0) ? (int)std::min<uint64_t>(std::max<uint64_t>((w.n_units + PB_NWARPS - 1) / PB_NWARPS, 1), max_ctas) : 0;
-      if (rp.agg_kind >= 3) wl.grid_agg = (int)std::min<uint64_t>(std::max<uint64_t>((w.n_docs + PB_AGG_SMEM_THREADS - 1) / PB_AGG_SMEM_THREADS, 1), (uint64_t)ctx->num_sms);
-      else if (rp.agg_kind) wl.grid_agg = (int)std::min<uint64_t>(std::max<uint64_t>((w.n_docs + PB_NTHREADS - 1) / PB_NTHREADS, 1), max2);
-      if (w.n_docs == 0) wl.grid_agg = 0;
-      rp.waves.push_back(wl);
-    }
-    // a plan can be kept for the next identical query when nothing about it depends on this call's circumstances: all
-    // segments resident (no staging waits, no in-place host reads), one wave, tables small enough for single-pass hand-back
-    bool small = true;
-    for (auto& tm : r->tables) if (tm.capacity + 1 > (1ull << 20)) small = false;
-    rp.cacheable = n_pending == 0 && !in_place && waves.size() == 1 && small && !(q->flags & PB_Q_DEFER_FINALIZE) && r->in_place_columns == 0;
+  rp.expand_items = P.d_expand_items; rp.n_expand = (int)P.expand_items.size();
+  rp.agg = P.n_docs_total == 0 ? AGG_NONE : P.d_row_segs ? AGG_ROWS : use_smem_table ? AGG_SMEM : AGG_GENERAL;
+  const bool smem_threads = rp.agg == AGG_SMEM || rp.agg == AGG_ROWS;   // PB_AGG_SMEM_THREADS per CTA, one CTA per SM
+  rp.smem_agg = (use_smem_table && smem_threads) ? (size_t)P.st_replicas * P.st_rep_bytes : rp.agg == AGG_ROWS ? 0 : smem2;
+  rp.row_segs = P.d_row_segs; rp.rows_rw = P.rows_rw;
+  rp.lane_w = P.d_lane_w; rp.n_lanes = 1 + P.nF; rp.n_segs = P.n_segs;
+  for (auto& wl : rp.waves) {
+    // every CTA gets a contiguous range of chunks; keep at least one chunk per warp
+    wl.grid_filter = (!P.match_all && wl.n_units > 0) ? (int)std::min<uint64_t>(std::max<uint64_t>((wl.n_units + PB_NWARPS - 1) / PB_NWARPS, 1), max_ctas) : 0;
+    if (wl.n_docs == 0 || rp.agg == AGG_NONE) wl.grid_agg = 0;
+    else if (smem_threads) wl.grid_agg = (int)std::min<uint64_t>(std::max<uint64_t>((wl.n_docs + PB_AGG_SMEM_THREADS - 1) / PB_AGG_SMEM_THREADS, 1), (uint64_t)ctx->num_sms);
+    else wl.grid_agg = (int)std::min<uint64_t>(std::max<uint64_t>((wl.n_docs + PB_NTHREADS - 1) / PB_NTHREADS, 1), max2);
   }
-  if ((rc = enqueue_all(r, &seg_wait))) return rc;
+  // a plan can be kept for the next identical query when nothing about it depends on this call's circumstances: all
+  // segments resident (no staging waits, no in-place host reads), one wave, tables small enough for single-pass hand-back
+  bool small = true;
+  for (auto& tm : r->tables) if (tm.capacity + 1 > (1ull << 20)) small = false;
+  rp.cacheable = P.n_pending == 0 && !P.in_place && rp.waves.size() == 1 && small && !(P.q->flags & PB_Q_DEFER_FINALIZE) && r->in_place_columns == 0;
+  return PB_OK;
+}
+
+// One device's part of a query: every segment of `g` lives on g->ctx.  Leaves the tables on the device when
+// PB_Q_DEFER_FINALIZE is set; otherwise merges across ranks (PB_Q_ALL_RANKS) and finalizes.
+static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, const pb_query_desc* q, pb_result_handle* out) {
+  int rc = validate_query(g, sqs, q);
+  if (rc) return rc;
+
+  // ---- plan cache: the same query over the same segments again -> replay its parked plan ----
+  std::string sig;
+  const bool try_cache = plan_cache_enabled() && !(q->flags & (PB_Q_DEFER_FINALIZE | PB_Q_GATHER_IN_PLACE));
+  if (try_cache) {
+    sig = plan_signature(g, sqs, q);
+    if (pb_result_s* p = plan_take(g, sig)) {
+      if ((rc = replay_plan(p, q))) { free_result(p); return rc; }
+      *out = p;
+      return PB_OK;
+    }
+  }
+  Plan P;
+  P.g = g; P.sqs = sqs; P.q = q; P.ctx = g->ctx;
+  P.n_segs = (int)g->segs.size(); P.nG = q->num_group_by; P.nA = q->num_aggregations; P.nF = q->num_agg_filters;
+  P.combine = (q->flags & PB_Q_COMBINE) != 0;
+  P.in_place = (q->flags & PB_Q_GATHER_IN_PLACE) != 0;
+  P.n_tables = P.combine ? 1 : P.n_segs;
+  std::unique_ptr<pb_result_s, void (*)(pb_result_s*)> R(new pb_result_s(), free_result);
+  pb_result_s* r = P.r = R.get();
+  r->group = g; r->n_gb = P.nG; r->n_aggs = P.nA; r->combine = P.combine; r->ctx = P.ctx;
+  if ((rc = stream_set_acquire(P.ctx, &r->sset))) return rc;
+  r->stream = P.st = r->sset.stream;
+  r->ev0 = r->sset.ev[0]; r->ev1 = r->sset.ev[1]; r->evm = r->sset.ev[2]; r->ev2 = r->sset.ev[3]; r->ev3 = r->sset.ev[4];
+  for (int j = 0; j < P.nG; j++) r->gb_names.push_back(q->group_by_columns[j]);
+  for (int a = 0; a < P.nA; a++) {
+    r->agg_op.push_back(q->aggregations[a].op);
+    r->agg_cols.push_back(q->aggregations[a].column ? q->aggregations[a].column : "");
+  }
+  r->n_agg_filters = P.nF; r->count_all = (q->flags & PB_Q_NULL_HANDLING) != 0;
+  if (P.nF > 0) r->agg_filter_of.assign(q->agg_filter_of, q->agg_filter_of + P.nA);
+
+  double t_prev = now_us();
+  auto lap = [&](int i) { double t = now_us(); r->host_us[i] += t - t_prev; t_prev = t; };
+  if ((rc = stage_inputs(P))) return rc;
+  lap(0);
+  if ((rc = plan_table_mode(P)) || (rc = alloc_tables(P))) return rc;
+  lap(1);
+  if ((rc = alloc_arena(P))) return rc;
+  for (int si = 0; si < P.n_segs; si++) if ((rc = bind_segment(P, si))) return rc;
+  if ((rc = plan_rows_kernel(P)) || (rc = plan_units(P)) || (rc = plan_match_path(P)) || (rc = fill_counters_head(P)) ||
+      (rc = plan_lane_weights(P))) return rc;
+  fill_query(P);
+  if ((rc = put_expand_items(P)) || (rc = plan_waves(P)) || (rc = upload_descriptors(P))) return rc;
+  lap(2);
+  if ((rc = plan_launches(P)) || (rc = enqueue_all(r, &P.seg_wait))) return rc;
   lap(3);
 
   if (q->flags & PB_Q_DEFER_FINALIZE) {
-    CU(cudaEventRecord(r->ev3, st));
+    CU(cudaEventRecord(r->ev3, P.st));
     *out = R.release();
     return PB_OK;
   }

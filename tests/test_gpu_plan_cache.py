@@ -32,8 +32,8 @@ def _queries(segs):
     d3 = segs[0].columns["c3"].dictionary_values()
     k2, k3 = int(d2[len(d2) // 2]), int(d3[len(d3) // 3])
     return [
-        datagen.config2_sql(segs, 16),                                                        # selective: fused aggregation
-        datagen.config2_sql(segs, 500),                                                       # 25 %: shared-memory table
+        datagen.config2_sql(segs, 16),                                                        # selective: row-group aggregation
+        datagen.config2_sql(segs, 500),                                                       # 25 %: row-group aggregation
         f"SELECT COUNT(*), SUM(m0), MIN(m1), MAX(m2) FROM t WHERE c2 < {k2}",                 # keyless
         f"SELECT d0, DISTINCTCOUNT(c3), SUM(m1) FROM t WHERE c2 < {k2} GROUP BY d0 LIMIT 100000",
         f"SELECT d1, SUM(m0) FILTER(WHERE c3 < {k3}), COUNT(*) FILTER(WHERE c3 < {k3}), COUNT(*) FROM t WHERE c2 < {k2} GROUP BY d1 LIMIT 100000",
