@@ -275,6 +275,19 @@ int pb_result_phase_ms(pb_result_handle r, double* filter_kernel_ms, double* agg
 int32_t pb_result_kernel_launches(pb_result_handle r);
 double pb_result_comm_ms(pb_result_handle r);           /* device time of the cross-rank merge (collective + merge kernel) */
 int32_t pb_result_in_place_columns(pb_result_handle r);   /* (segment, column) pairs this query gathered in place from host memory */
+/* The kernels this call was planned onto (testing): fills out[0 .. min(n, PB_PLAN_INFO_N)) and returns the number filled
+ * (0 for a multi-device shell result).  A plan-cache replay reports the plan it replays.
+ *   [0] aggregation kernel: 0 none (no docs), 1 pb_agg_kernel, 2 pb_agg_smem_kernel, 3 pb_agg_rows_kernel
+ *   [1] pb_agg_rows_kernel row width RW in 32-bit words (0: not that kernel)
+ *   [2] replicas of the CTA-private shared-memory table (0: none planned)   [3] its st_min_docs, clamped to INT32_MAX
+ *   [4] table mode: 0 keyless, 1 dense, 2 hash                              [5] hash key words (1 or 2)
+ *   [6] filter kernel: 0 none (match all), 1 general U=1, 2 general U=2, 3 specialised
+ *   [7] specialised filter kernel: dictId width W   [8] its predicate kind K (0 range, 1 set)
+ *   [9] 1 when some segment evaluates a scan leaf on candidates only
+ *   [10] bit mask of the aggregations pb_agg_rows_kernel sums as exact 64-bit integers in the CTA-private table (0 without
+ *        one); the kernel takes that table, and so these sums, when the launch has at least st_min_docs matches */
+#define PB_PLAN_INFO_N 11
+int32_t pb_result_plan_info(pb_result_handle r, int32_t* out, int32_t n);
 /* host-side microseconds spent in this call, by phase: [0] resolve + stage, [1] table allocation + init,
  * [2] descriptor build + upload, [3] kernel launches, [4] wait for the scan + group count, [5] compaction,
  * gathers and read-back, [6] host key decode / stats; [7] reserved */

@@ -1065,6 +1065,7 @@ struct pb_result_s {
   struct InitArgs { uint4* zero = nullptr; uint64_t zn = 0; uint4* ff = nullptr; uint64_t fn = 0; uint4* mm = nullptr; uint64_t mn = 0;
                     uint4* aux = nullptr; uint64_t an = 0; const uint4* head = nullptr; uint64_t head_n16 = 0; int grid = 1; } init;   // pb_init_tables_kernel
   int key_words = 1;
+  int32_t plan_info[PB_PLAN_INFO_N] = {0};  // pb_result_plan_info, filled by plan_launches
   // ORDER BY ... LIMIT trim (pb_query_desc.order_by): per table an order-key array and the radix-select state
   pb_order_by order0{0, 0, 0}; int trim_size = 0, trim_threshold = 0;
   std::vector<unsigned long long*> d_okey; std::vector<DevSelectState*> d_sel;
@@ -2669,9 +2670,13 @@ static int plan_launches(Plan& P) {
       CU(cudaFuncSetAttribute(pb_filter_kernel<2, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       CU(cudaFuncSetAttribute(pb_agg_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
       CU(cudaFuncSetAttribute(pb_agg_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 16 * 1024));
-      CU(cudaFuncSetAttribute(pb_agg_rows_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 32 * 1024));
-      CU(cudaFuncSetAttribute(pb_agg_rows_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 32 * 1024));
-      CU(cudaFuncSetAttribute(pb_agg_rows_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 32 * 1024));
+      // the rows kernels: whatever their static shared memory (~20 KB of segment descriptors) leaves -- a CTA table of the
+      // whole 200 KB budget must fit (227 - 32 KB refused tables of 195 .. 200 KB with an invalid-argument launch error)
+      for (const void* k : {(const void*)pb_agg_rows_kernel<2>, (const void*)pb_agg_rows_kernel<4>, (const void*)pb_agg_rows_kernel<8>}) {
+        cudaFuncAttributes fa;
+        CU(cudaFuncGetAttributes(&fa, k));
+        CU(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)fa.sharedSizeBytes));
+      }
       ctx->smem_attr_set = true;
     }
   }
@@ -2720,6 +2725,16 @@ static int plan_launches(Plan& P) {
   bool small = true;
   for (auto& tm : r->tables) if (tm.capacity + 1 > (1ull << 20)) small = false;
   rp.cacheable = P.n_pending == 0 && !P.in_place && rp.waves.size() == 1 && small && !(P.q->flags & PB_Q_DEFER_FINALIZE) && r->in_place_columns == 0;
+  int32_t* pi = r->plan_info;
+  pi[0] = (int32_t)rp.agg; pi[1] = rp.agg == AGG_ROWS ? rp.rows_rw : 0;
+  pi[2] = P.st_replicas; pi[3] = P.st_replicas > 0 ? (int32_t)std::min<uint64_t>(P.hq->st_min_docs, INT32_MAX) : 0;
+  pi[4] = r->table_mode; pi[5] = r->key_words;
+  pi[6] = (P.match_all || P.n_chunks == 0) ? 0 : rp.spec_w > 0 ? 3 : rp.U;
+  pi[7] = rp.spec_w; pi[8] = rp.spec_w > 0 ? rp.spec_pk : 0;
+  pi[9] = P.any_cand_leaf ? 1 : 0;
+  pi[10] = 0;
+  // (the rows kernel sums exactly only in the CTA-private table: without one the flag is not used)
+  if (P.h_row_segs && P.st_replicas > 0) for (int a = 0; a < P.nA; a++) if (P.h_row_segs[0].aggs[a].exact_int) pi[10] |= 1 << a;
   return PB_OK;
 }
 
@@ -3252,6 +3267,12 @@ extern "C" double pb_result_scan_kernel_ms(pb_result_handle r) {
   return r->scan_ms;
 }
 extern "C" int32_t pb_result_kernel_launches(pb_result_handle r) { return r ? r->launches : 0; }
+extern "C" int32_t pb_result_plan_info(pb_result_handle r, int32_t* out, int32_t n) {
+  if (!r || !out || !r->parts.empty()) return 0;
+  const int32_t k = std::min<int32_t>(std::max<int32_t>(n, 0), PB_PLAN_INFO_N);
+  for (int32_t i = 0; i < k; i++) out[i] = r->plan_info[i];
+  return k;
+}
 extern "C" void* pb_result_stream(pb_result_handle r) { return r ? (void*)r->stream : nullptr; }
 
 

@@ -24,6 +24,10 @@ PB_Q_NO_TMA = 8
 PB_Q_GATHER_IN_PLACE = 16
 PB_Q_ALL_RANKS = 32
 PB_COMM_ID_BYTES = 128
+# pb_result_plan_info, in order.  agg_kernel: 0 none, 1 general, 2 smem table, 3 rows; table_mode: 0 keyless, 1 dense,
+# 2 hash; filter_kernel: 0 none, 1 general U=1, 2 general U=2, 3 specialised (spec_w, spec_k)
+PLAN_INFO_FIELDS = ("agg_kernel", "rows_rw", "st_replicas", "st_min_docs", "table_mode", "key_words", "filter_kernel",
+                    "spec_w", "spec_k", "cand_leaf", "exact_int_mask")
 
 
 class PbColumnDesc(C.Structure):
@@ -151,6 +155,8 @@ def lib():
     l.pb_result_kernel_launches.restype = C.c_int32
     l.pb_result_in_place_columns.argtypes = [C.c_void_p]
     l.pb_result_in_place_columns.restype = C.c_int32
+    l.pb_result_plan_info.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]
+    l.pb_result_plan_info.restype = C.c_int32
     l.pb_result_stream.argtypes = [C.c_void_p]
     l.pb_result_stream.restype = C.c_void_p
     l.pb_result_wait.argtypes = [C.c_void_p]
@@ -425,6 +431,13 @@ class Result:
         self.scan_kernel_ms = l.pb_result_scan_kernel_ms(self._rh)
         self.kernel_launches = l.pb_result_kernel_launches(self._rh)
         self.in_place_columns = l.pb_result_in_place_columns(self._rh)
+
+    @property
+    def plan_info(self) -> Dict[str, int]:
+        """The kernels the call was planned onto (pb_result_plan_info; testing).  Empty for a multi-device result."""
+        arr = (C.c_int32 * len(PLAN_INFO_FIELDS))()
+        n = lib().pb_result_plan_info(self._rh, arr, len(arr))
+        return dict(zip(PLAN_INFO_FIELDS[:n], list(arr)[:n]))
 
     def device_buffer(self, which: int, agg: int = 0):
         p, n = C.c_void_p(), C.c_int64()

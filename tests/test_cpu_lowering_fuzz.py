@@ -11,23 +11,8 @@ import pytest
 from oracle import oracle
 from pinot_b200 import datagen, native
 from pinot_b200.query import parse_sql
-from pinot_b200.segment_writer import DataType, unpack_bits_be
-
-
-def _dict_ids(c):
-    if c.is_sorted:
-        pairs = np.frombuffer(c.forward_index.tobytes(), dtype=">i4").reshape(-1, 2)
-        ids = np.zeros(c.num_docs, np.int64)
-        for d, (s, e) in enumerate(pairs):
-            ids[s:e + 1] = d
-        return ids
-    return unpack_bits_be(c.forward_index, c.num_docs, c.bits_per_element).astype(np.int64)
-
-
-def _raw_values(c):
-    dt = {DataType.INT: ">i4", DataType.LONG: ">i8", DataType.FLOAT: ">f4", DataType.DOUBLE: ">f8"}[c.data_type]
-    width = np.dtype(dt).itemsize
-    return np.frombuffer(c.forward_index.tobytes()[-width * c.num_docs:], dtype=dt)
+from pinot_b200.segment_writer import DataType
+from tests.reference import _column_values, _dict_ids, _raw_values, evaluate_sql  # noqa: F401  (shared with other tests)
 
 
 def evaluate_lowered(seg, lines):
@@ -85,58 +70,6 @@ def evaluate_lowered(seg, lines):
             raise AssertionError(f"unknown node {line!r}")
     assert len(stack) == 1
     return stack[0]
-
-
-def _column_values(seg, col):
-    c = seg.columns[col]
-    if not c.has_dictionary:
-        v = _raw_values(c)
-        return v.astype(np.float64) if c.data_type in (DataType.FLOAT, DataType.DOUBLE) else v.astype(np.int64)
-    d = c.dictionary_values()
-    ids = _dict_ids(c)
-    if c.data_type == DataType.STRING:
-        return np.array(list(d), dtype="S")[ids]                     # bytes: same order as Java compareTo for ASCII
-    return d.astype(np.int64)[ids] if c.data_type in (DataType.INT, DataType.LONG) else d.astype(np.float64)[ids]
-
-
-def evaluate_sql(seg, node):
-    """Third opinion: the WHERE tree straight from the SQL semantics on the decoded column values (no dictIds, no indexes)."""
-    from pinot_b200.query import And, Not, Or, PredicateType
-    if isinstance(node, (And, Or)):
-        parts = [evaluate_sql(seg, c) for c in node.children]
-        return np.logical_and.reduce(parts) if isinstance(node, And) else np.logical_or.reduce(parts)
-    if isinstance(node, Not):
-        return ~evaluate_sql(seg, node.child)
-    c = seg.columns[node.column]
-    v = _column_values(seg, node.column)
-
-    def lit(s):
-        if c.data_type == DataType.STRING:
-            return s.encode()
-        return float(s) if c.data_type in (DataType.FLOAT, DataType.DOUBLE) else int(s)
-
-    def cmp(op, x):
-        return op(v, np.bytes_(x)) if c.data_type == DataType.STRING else op(v, x)
-    import operator as o
-    t = node.type
-    if t in (PredicateType.EQ, PredicateType.NOT_EQ):
-        m = cmp(o.eq, lit(node.values[0]))
-        return ~m if t == PredicateType.NOT_EQ else m
-    if t in (PredicateType.IN, PredicateType.NOT_IN):
-        if not c.has_dictionary and c.data_type in (DataType.FLOAT, DataType.DOUBLE):
-            # a fastutil DoubleSet compares Double.doubleToLongBits (-0.0 is not in {0.0}); EQ / NOT_EQ above compare with ==
-            bits = v.astype(np.float64).view(np.int64)
-            lits = [np.float32(x) if c.data_type == DataType.FLOAT else np.float64(x) for x in node.values]
-            m = np.isin(bits, np.array([np.float64(x) for x in lits]).view(np.int64))
-        else:
-            m = np.logical_or.reduce([cmp(o.eq, lit(x)) for x in node.values])
-        return ~m if t == PredicateType.NOT_IN else m
-    m = np.ones(seg.num_docs, bool)
-    if node.lower is not None:
-        m &= cmp(o.ge if node.lower_inclusive else o.gt, lit(node.lower))
-    if node.upper is not None:
-        m &= cmp(o.le if node.upper_inclusive else o.lt, lit(node.upper))
-    return m
 
 
 @pytest.fixture(scope="module")
