@@ -285,8 +285,10 @@ int32_t pb_result_in_place_columns(pb_result_handle r);   /* (segment, column) p
  *   [7] specialised filter kernel: dictId width W   [8] its predicate kind K (0 range, 1 set)
  *   [9] 1 when some segment evaluates a scan leaf on candidates only
  *   [10] bit mask of the aggregations pb_agg_rows_kernel sums as exact 64-bit integers in the CTA-private table (0 without
- *        one); the kernel takes that table, and so these sums, when the launch has at least st_min_docs matches */
-#define PB_PLAN_INFO_N 11
+ *        one); the kernel takes that table, and so these sums, when the launch has at least st_min_docs matches
+ *   [11] 1 when the specialised filter kernel aggregates its own survivors (no match list, no aggregation kernel); [0], [1],
+ *        [2] and [10] then describe the pb_agg_rows_kernel path it replaces: 3, the row width, 0 and 0 */
+#define PB_PLAN_INFO_N 12
 int32_t pb_result_plan_info(pb_result_handle r, int32_t* out, int32_t n);
 /* host-side microseconds spent in this call, by phase: [0] resolve + stage, [1] table allocation + init,
  * [2] descriptor build + upload, [3] kernel launches, [4] wait for the scan + group count, [5] compaction,

@@ -169,6 +169,7 @@ struct DevTable {
   uint32_t limit_active;             // 0: the table can never reach numGroupsLimit (limit >= docs), inserts need no ticket
 };
 
+struct DevRowSeg;
 struct DevQuery {
   int32_t n_segs;
   int32_t n_group_by;
@@ -200,6 +201,7 @@ struct DevQuery {
   const unsigned int* any_limit;         // see DevTable::any_limit
   const DevSegQuery* segs;
   DevTable* tables;
+  const DevRowSeg* row_segs;             // fused filter kernel (RW > 0): per segment, the row group its candidate round aggregates from
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -482,20 +484,21 @@ static __device__ __noinline__ uint32_t pb_eval_raw(const uint32_t* __restrict__
   return mine;
 }
 
+// dictId `id` against an L_DICT_RANGE / L_DICT_SET leaf
+__device__ __forceinline__ bool pb_dict_leaf_test(const DevLeaf& lf, const uint8_t* __restrict__ set_cache, uint32_t id) {
+  if (lf.kind == L_DICT_RANGE) return (id - lf.lo) < lf.span;
+  if (lf.set_smem_off >= 0) return set_cache[lf.set_smem_off + id] != 0;         // exclusive flag folded in
+  return (((__ldg(lf.set_bits + (id >> 5)) >> (id & 31)) & 1u) ^ (uint32_t)lf.exclusive) != 0;
+}
+
 // one doc against one scan leaf, reading the forward index in place (candidate evaluation, see DevLeaf::gather)
 __device__ __forceinline__ bool pb_leaf_test_doc(const DevLeaf& lf, const uint8_t* __restrict__ set_cache, uint32_t doc) {
   switch (lf.kind) {
     case L_TRUE: return true;
     case L_FALSE: return false;
-    case L_DICT_RANGE: {
-      const uint32_t id = pb_unpack_at_bounded(lf.gfwd, doc, lf.bits, lf.g_full_words, lf.g_tail_word, lf.g_stride_bits, lf.g_bit_off);
-      return (id - lf.lo) < lf.span;
-    }
-    case L_DICT_SET: {
-      const uint32_t id = pb_unpack_at_bounded(lf.gfwd, doc, lf.bits, lf.g_full_words, lf.g_tail_word, lf.g_stride_bits, lf.g_bit_off);
-      if (lf.set_smem_off >= 0) return set_cache[lf.set_smem_off + id] != 0;         // exclusive flag folded in
-      return (((__ldg(lf.set_bits + (id >> 5)) >> (id & 31)) & 1u) ^ (uint32_t)lf.exclusive) != 0;
-    }
+    case L_DICT_RANGE:
+    case L_DICT_SET:
+      return pb_dict_leaf_test(lf, set_cache, pb_unpack_at_bounded(lf.gfwd, doc, lf.bits, lf.g_full_words, lf.g_tail_word, lf.g_stride_bits, lf.g_bit_off));
     case L_BITMAP: return (((__ldg(lf.bitmap + (doc >> 5)) >> (doc & 31)) & 1u) ^ (uint32_t)lf.exclusive) != 0;
     case L_RAW_RANGE_I: { const long long v = pb_raw_i64(lf.gfwd, doc, lf.raw_width, lf.data_type, lf.g_stride_bits, lf.g_bit_off); return v >= lf.ilo && v <= lf.ihi; }
     case L_RAW_RANGE_F: {
@@ -846,6 +849,90 @@ __device__ __forceinline__ void pb_accumulate_smem(const DevQuery& Q, const DevS
 }
 
 // ------------------------------------------------------------------------------------------------
+// One row of a row group taken apart in registers: what pb_agg_rows_kernel does per matching doc, and what the fused
+// candidate round of pb_filter_kernel does per surviving candidate.  RW = 32-bit words per row.
+// ------------------------------------------------------------------------------------------------
+struct DevRowKey { uint32_t off, bits; uint64_t mult; const int32_t* remap; };
+struct DevRowAgg { uint32_t off, width, type, exact_int; };  // width 4 / 8 bytes, type PB_INT .. PB_DOUBLE; unused for COUNT(*).  exact_int: SUM / AVG
+                                                             // of an integer column whose sums stay below 2^53 (same flag in every segment)
+struct DevRowSeg {
+  const uint32_t* rows;
+  uint64_t doc_base;
+  int32_t table, pad;
+  DevRowKey keys[PB_MAX_GROUP_BY];
+  DevRowAgg aggs[PB_MAX_AGGS];
+};
+
+// row `doc` (inside its segment) with one vector load -- rows never straddle a 32-byte sector -- byte-swapped to MSB-first words
+template <int RW>
+__device__ __forceinline__ void pb_load_row(const uint32_t* __restrict__ rows, unsigned long long doc, uint32_t (&w)[RW]) {
+  const uint32_t* __restrict__ row = rows + doc * (unsigned long long)RW;
+  if (RW == 2) { const uint2 v = __ldg(reinterpret_cast<const uint2*>(row)); w[0] = v.x; w[1 % RW] = v.y; }
+  else {
+#pragma unroll
+    for (int q4 = 0; q4 < RW / 4; q4++) {
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(row) + q4);
+      w[(4 * q4) % RW] = v.x; w[(4 * q4 + 1) % RW] = v.y; w[(4 * q4 + 2) % RW] = v.z; w[(4 * q4 + 3) % RW] = v.w;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < RW; k++) w[k] = pb_bswap32(w[k]);
+}
+
+// the `bits`-bit field at bit `off` of a loaded row
+template <int RW>
+__device__ __forceinline__ uint32_t pb_row_field(const uint32_t (&w)[RW], uint32_t off, uint32_t bits) {
+  const uint32_t wi = off >> 5, sh = off & 31u;
+  uint32_t hi = w[0], lo = RW > 1 ? w[1 % RW] : 0u;
+#pragma unroll
+  for (int k = 1; k < RW; k++) if (wi == (uint32_t)k) { hi = w[k]; lo = k + 1 < RW ? w[(k + 1) % RW] : 0u; }
+  return __funnelshift_l(lo, hi, sh) >> (32u - bits);
+}
+
+// dense slot of the row: key dictIds -> (remap to the global dictionary) -> mixed radix
+template <int RW>
+__device__ __forceinline__ uint64_t pb_row_slot(const uint32_t (&w)[RW], const DevRowSeg& sg, int nG) {
+  uint64_t slot = 0;
+  for (int j = 0; j < nG; j++) {
+    const DevRowKey& k = sg.keys[j];
+    uint32_t id = pb_row_field<RW>(w, k.off, k.bits);
+    if (k.remap) id = (uint32_t)__ldg(k.remap + id);
+    slot += (uint64_t)id * k.mult;
+  }
+  return slot;
+}
+
+// the row's value field of an aggregation, widened to double like BlockValSet.getDoubleValuesSV
+template <int RW>
+__device__ __forceinline__ double pb_row_value(const uint32_t (&w)[RW], const DevRowAgg& g) {
+  const uint32_t w0 = pb_row_field<RW>(w, g.off, 32u);
+  if (g.width == 4) return g.type == 2 ? (double)__uint_as_float(w0) : (double)(int32_t)w0;
+  const unsigned long long u = ((unsigned long long)w0 << 32) | pb_row_field<RW>(w, g.off + 32u, 32u);
+  return g.type == 3 ? __longlong_as_double((long long)u) : (double)(long long)u;
+}
+template <int RW>
+__device__ __forceinline__ long long pb_row_ivalue(const uint32_t (&w)[RW], const DevRowAgg& g) {   // INT / LONG fields only
+  const uint32_t w0 = pb_row_field<RW>(w, g.off, 32u);
+  if (g.width == 4) return (long long)(int32_t)w0;
+  return (long long)(((unsigned long long)w0 << 32) | pb_row_field<RW>(w, g.off + 32u, 32u));
+}
+
+// a matching row straight into the global table of its segment: fire-and-forget reductions.  doc: inside the segment
+template <int RW>
+__device__ __forceinline__ void pb_row_aggregate_global(const DevQuery& Q, const DevRowSeg& sg, const uint32_t (&w)[RW], uint64_t slot, uint32_t doc) {
+  const DevTable& t = Q.tables[sg.table];
+  pb_red_add_u64(&t.rowcnt[slot], 1ull);
+  if (t.first_doc) asm volatile("red.global.min.u32 [%0], %1;" ::"l"(t.first_doc + slot), "r"(doc));
+  for (int a = 0; a < Q.n_aggs; a++) {
+    const int op = Q.agg_op[a];
+    if (op == 0) continue;
+    const double v = pb_row_value<RW>(w, sg.aggs[a]);
+    if (op == 1 || op == 4) pb_red_add_f64(&t.sum[a][slot], v);
+    else if (v == v) pb_red_min_s64(&t.mm[a][slot], op == 2 ? pb_enc_f64(v) : ~pb_enc_f64(v));   // (few matches: a read-before-RED would only add a dependent L2 round trip)
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Kernel 1: pb_filter_kernel  (DocIdSetOperator + filter operators: SURVEY.md §3.2)
 //
 // A CTA owns a contiguous range of 1024-doc chunks; inside it every WARP is an independent worker with its
@@ -874,12 +961,19 @@ struct __align__(16) FilterSmemHeader {
 // dictionary column of SW bits tested with predicate kind SPK (0 = dictId range, 1 = IN / NOT IN membership LUT), every
 // other leaf evaluated on the candidates -- with that leaf's unpack + test inlined and nothing else compiled in.  The host
 // picks it when every segment of the launch has that shape (pb_filter_spec.cu holds the instantiations).
-template <int U, int MIN_CTAS, int SW = 0, int SPK = 0>
+//
+// RW > 0 (specialised kernels only): the FUSED variant for a selective dense group-by over row groups of RW words.  The
+// candidate round loads each candidate's whole row once (the sector the candidate leaves read anyway), tests every
+// candidate leaf from those registers and sends a survivor straight into the global group table the way
+// pb_agg_rows_kernel's global path does.  No match list is written and no aggregation kernel runs.
+template <int U, int MIN_CTAS, int SW = 0, int SPK = 0, int RW = 0>
 __global__ void __launch_bounds__(PB_NTHREADS, MIN_CTAS) pb_filter_kernel(const __grid_constant__ DevQuery Q) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   FilterSmemHeader* H = reinterpret_cast<FilterSmemHeader*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   uint8_t* dyn = smem_raw + ((sizeof(FilterSmemHeader) + 127) & ~(size_t)127);
+  DevRowSeg* rseg = reinterpret_cast<DevRowSeg*>(dyn);   // RW > 0: the current segment's row-group descriptor
+  if constexpr (RW > 0) dyn += (sizeof(DevRowSeg) + 127) & ~(size_t)127;
   uint8_t* set_cache = dyn;
   dyn += (Q.set_cache_bytes + 127) & ~127;
   uint16_t* cand = reinterpret_cast<uint16_t*>(dyn);     // per-warp candidate lists (only when some leaf is evaluated on candidates)
@@ -970,6 +1064,11 @@ __global__ void __launch_bounds__(PB_NTHREADS, MIN_CTAS) pb_filter_kernel(const 
       const uint32_t* src = reinterpret_cast<const uint32_t*>(&Q.segs[sgi]);
       uint32_t* dst = reinterpret_cast<uint32_t*>(H->seg);
       for (int i = tid; i < (int)(PB_SEG_FILTER_BYTES / 4); i += PB_NTHREADS) dst[i] = src[i];
+      if constexpr (RW > 0) {
+        const uint32_t* rsrc = reinterpret_cast<const uint32_t*>(Q.row_segs + sgi);
+        uint32_t* rdst = reinterpret_cast<uint32_t*>(rseg);
+        for (int i = tid; i < (int)(sizeof(DevRowSeg) / 4); i += PB_NTHREADS) rdst[i] = rsrc[i];
+      }
       __syncthreads();
       if (tid < sq.n_scan) {
         const uint32_t stride = (uint32_t)(UNIT_DOCS / 8) * (uint32_t)sq.scan[tid].bits_per_doc;
@@ -1167,7 +1266,7 @@ __global__ void __launch_bounds__(PB_NTHREADS, MIN_CTAS) pb_filter_kernel(const 
         excl = incl - cnt;
       }
       const uint32_t gunit0 = (uint32_t)(sq.doc_base + unit_doc0);
-      if (n_cand_leaves == 0) {
+      if (RW == 0 && n_cand_leaves == 0) {     // (the fused kernel takes every survivor through the candidate round)
         if (__builtin_expect(total > OUT_CAP, 0)) {
           // dense matches: straight to the list
           unsigned long long base = 0;
@@ -1227,17 +1326,28 @@ __global__ void __launch_bounds__(PB_NTHREADS, MIN_CTAS) pb_filter_kernel(const 
             bool alive = idx < n_pass;
             const uint32_t off = alive ? (uint32_t)cl[idx] : 0u;
             const uint32_t doc = (uint32_t)unit_doc0 + off;          // doc inside the segment
-            for (int i = 0; i < n_cand_leaves; i++) {
-              if (alive) alive = pb_leaf_test_doc(sq.leaves[H->flat_leaf[H->n_dense + i]], set_cache, doc);
-              if (!__any_sync(0xffffffffu, alive)) break;
-            }
-            const uint32_t bal = __ballot_sync(0xffffffffu, alive);
-            if (bal) {
-              const uint32_t n = (uint32_t)__popc(bal);
-              if (out_n + n > OUT_CAP) flush_out();
-              if (alive) ob[out_n + __popc(bal & lt)] = gunit0 + off;
-              out_n += n;
-              matched += n;
+            if constexpr (RW > 0) {
+              uint32_t w[RW];
+              if (alive) pb_load_row<RW>(rseg->rows, doc, w);
+              for (int i = 0; i < n_cand_leaves; i++) {
+                const DevLeaf& lf = sq.leaves[H->flat_leaf[H->n_dense + i]];
+                if (alive) alive = pb_dict_leaf_test(lf, set_cache, pb_row_field<RW>(w, (uint32_t)lf.g_bit_off, (uint32_t)lf.bits));
+              }
+              if (alive) pb_row_aggregate_global<RW>(Q, *rseg, w, pb_row_slot<RW>(w, *rseg, Q.n_group_by), doc);
+              matched += (uint32_t)__popc(__ballot_sync(0xffffffffu, alive));
+            } else {
+              for (int i = 0; i < n_cand_leaves; i++) {
+                if (alive) alive = pb_leaf_test_doc(sq.leaves[H->flat_leaf[H->n_dense + i]], set_cache, doc);
+                if (!__any_sync(0xffffffffu, alive)) break;
+              }
+              const uint32_t bal = __ballot_sync(0xffffffffu, alive);
+              if (bal) {
+                const uint32_t n = (uint32_t)__popc(bal);
+                if (out_n + n > OUT_CAP) flush_out();
+                if (alive) ob[out_n + __popc(bal & lt)] = gunit0 + off;
+                out_n += n;
+                matched += n;
+              }
             }
           }
         }
@@ -1511,16 +1621,6 @@ static __global__ void __launch_bounds__(PB_AGG_SMEM_THREADS, 1) pb_agg_smem_ker
 // Table update: the CTA-private shared-memory table (SmemTable) when the launch carries one and has enough matches, else
 // reductions into the global table.
 // ------------------------------------------------------------------------------------------------
-struct DevRowKey { uint32_t off, bits; uint64_t mult; const int32_t* remap; };
-struct DevRowAgg { uint32_t off, width, type, exact_int; };  // width 4 / 8 bytes, type PB_INT .. PB_DOUBLE; unused for COUNT(*).  exact_int: SUM / AVG
-                                                             // of an integer column whose sums stay below 2^53 (same flag in every segment)
-struct DevRowSeg {
-  const uint32_t* rows;
-  uint64_t doc_base;
-  int32_t table, pad;
-  DevRowKey keys[PB_MAX_GROUP_BY];
-  DevRowAgg aggs[PB_MAX_AGGS];
-};
 #define PB_ROWS_SMEM_SEGS 16
 
 template <int RW>
@@ -1572,46 +1672,19 @@ __global__ void __launch_bounds__(PB_AGG_SMEM_THREADS, 1) pb_agg_rows_kernel(con
   // the aggregation is latency-bound (most warps wait on memory when every field is its own load),
   // so the chain per doc is kept at match list -> row -> remap, and every thread works on two docs at a time.
   auto process = [&](unsigned long long gdoc, const uint32_t (&w)[RW], const DevRowSeg& sg) {
-    auto field = [&](uint32_t off, uint32_t bits) -> uint32_t {
-      const uint32_t wi = off >> 5, sh = off & 31u;
-      uint32_t hi = w[0], lo = RW > 1 ? w[1 % RW] : 0u;
-#pragma unroll
-      for (int k = 1; k < RW; k++) if (wi == (uint32_t)k) { hi = w[k]; lo = k + 1 < RW ? w[(k + 1) % RW] : 0u; }
-      return __funnelshift_l(lo, hi, sh) >> (32u - bits);
-    };
-    uint64_t slot = 0;
-    for (int j = 0; j < nG; j++) {
-      const DevRowKey& k = sg.keys[j];
-      uint32_t id = field(k.off, k.bits);
-      if (k.remap) id = (uint32_t)__ldg(k.remap + id);
-      slot += (uint64_t)id * k.mult;
-    }
-    // the row's value field of aggregation a, widened to double like BlockValSet.getDoubleValuesSV
-    auto value_of = [&](int a) -> double {
-      const DevRowAgg& g = sg.aggs[a];
-      const uint32_t w0 = field(g.off, 32u);
-      if (g.width == 4) return g.type == 2 ? (double)__uint_as_float(w0) : (double)(int32_t)w0;
-      const unsigned long long u = ((unsigned long long)w0 << 32) | field(g.off + 32u, 32u);
-      return g.type == 3 ? __longlong_as_double((long long)u) : (double)(long long)u;
-    };
-    auto ivalue_of = [&](int a) -> long long {           // INT / LONG fields only
-      const DevRowAgg& g = sg.aggs[a];
-      const uint32_t w0 = field(g.off, 32u);
-      if (g.width == 4) return (long long)(int32_t)w0;
-      return (long long)(((unsigned long long)w0 << 32) | field(g.off + 32u, 32u));
-    };
+    const uint64_t slot = pb_row_slot<RW>(w, sg, nG);
     if (use_smem) {
       const uint32_t sl = (uint32_t)slot;
       pb_sh_add_u32(st.cnt(sl), 1u);
       for (int a = 0; a < nA; a++) {
         const int op = Q.agg_op[a];
         if (op == 0) continue;
-        const double v = ((op == 1 || op == 4) && sg.aggs[a].exact_int) ? 0.0 : value_of(a);
+        const double v = ((op == 1 || op == 4) && sg.aggs[a].exact_int) ? 0.0 : pb_row_value<RW>(w, sg.aggs[a]);
         const uint32_t cell = st.acc(st.acc_of[a], sl);
         if ((op == 1 || op == 4) && sg.aggs[a].exact_int) {
           // exact integer sum: the cell is an int64 kept as two u32 halves, low half first; the carry out of the low half
           // (seen in the value the returning add hands back) rides on the add to the high half -- two native ATOMS, no loop
-          const long long iv = ivalue_of(a);
+          const long long iv = pb_row_ivalue<RW>(w, sg.aggs[a]);
           const uint32_t vlo = (uint32_t)iv, vhi = (uint32_t)((unsigned long long)iv >> 32);
           uint32_t add_hi = vhi;
           if (vlo) { const uint32_t before = pb_sh_atom_add_u32(cell, vlo); add_hi += (before + vlo) < vlo ? 1u : 0u; }
@@ -1633,16 +1706,7 @@ __global__ void __launch_bounds__(PB_AGG_SMEM_THREADS, 1) pb_agg_rows_kernel(con
         }
       }
     } else {
-      const DevTable& t = Q.tables[sg.table];
-      pb_red_add_u64(&t.rowcnt[slot], 1ull);
-      if (t.first_doc) asm volatile("red.global.min.u32 [%0], %1;" ::"l"(t.first_doc + slot), "r"((uint32_t)(gdoc - sg.doc_base)));
-      for (int a = 0; a < nA; a++) {
-        const int op = Q.agg_op[a];
-        if (op == 0) continue;
-        const double v = value_of(a);
-        if (op == 1 || op == 4) pb_red_add_f64(&t.sum[a][slot], v);
-        else if (v == v) pb_red_min_s64(&t.mm[a][slot], op == 2 ? pb_enc_f64(v) : ~pb_enc_f64(v));   // (few matches: a read-before-RED would only add a dependent L2 round trip)
-      }
+      pb_row_aggregate_global<RW>(Q, sg, w, slot, (uint32_t)(gdoc - sg.doc_base));
     }
   };
   auto seg_of = [&](unsigned long long gdoc) -> int {
@@ -1654,19 +1718,6 @@ __global__ void __launch_bounds__(PB_AGG_SMEM_THREADS, 1) pb_agg_rows_kernel(con
     }
     return lo;
   };
-  auto load_row = [&](const DevRowSeg& sg, unsigned long long gdoc, uint32_t (&w)[RW]) {
-    const uint32_t* __restrict__ row = sg.rows + (gdoc - sg.doc_base) * (unsigned long long)RW;
-    if (RW == 2) { const uint2 v = __ldg(reinterpret_cast<const uint2*>(row)); w[0] = v.x; w[1 % RW] = v.y; }
-    else {
-#pragma unroll
-      for (int q4 = 0; q4 < RW / 4; q4++) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(row) + q4);
-        w[(4 * q4) % RW] = v.x; w[(4 * q4 + 1) % RW] = v.y; w[(4 * q4 + 2) % RW] = v.z; w[(4 * q4 + 3) % RW] = v.w;
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < RW; k++) w[k] = pb_bswap32(w[k]);
-  };
   const unsigned long long stride = (unsigned long long)gridDim.x * PB_AGG_SMEM_THREADS;
   for (unsigned long long i = (unsigned long long)blockIdx.x * PB_AGG_SMEM_THREADS + tid; i < n; i += 2 * stride) {
     const bool two = i + stride < n;
@@ -1675,8 +1726,8 @@ __global__ void __launch_bounds__(PB_AGG_SMEM_THREADS, 1) pb_agg_rows_kernel(con
     const DevRowSeg& sg0 = segs[seg_of(gdoc0)];
     const DevRowSeg& sg1 = segs[seg_of(gdoc1)];
     uint32_t w0[RW], w1[RW];
-    load_row(sg0, gdoc0, w0);
-    load_row(sg1, gdoc1, w1);
+    pb_load_row<RW>(sg0.rows, gdoc0 - sg0.doc_base, w0);
+    pb_load_row<RW>(sg1.rows, gdoc1 - sg1.doc_base, w1);
     process(gdoc0, w0, sg0);
     if (two) process(gdoc1, w1, sg1);
   }

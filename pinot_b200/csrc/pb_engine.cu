@@ -727,6 +727,7 @@ struct GlobalDict {
   int64_t n = 0;
   std::vector<uint8_t> values;                 // native-endian stored-type values / padded strings, sorted
   std::vector<std::vector<int32_t>> h_remap;   // per segment: local dictId -> global dictId
+  std::vector<char> identity;                  // per segment: h_remap[i] == i for every i, so the kernels need no remap
   std::vector<int32_t*> d_remap;
   uint8_t* d_values = nullptr;                 // device copy of `values`
   bool external = false;
@@ -884,6 +885,7 @@ static int upload_remaps(pb_group_s* g, GlobalDict& gd) {
 static int build_remaps(pb_group_s* g, const char* column, GlobalDict& gd) {
   gd.uploaded = false;
   gd.h_remap.assign(g->segs.size(), {});
+  gd.identity.assign(g->segs.size(), 0);
   std::vector<uint8_t> tmp((size_t)gd.entry_bytes);
   for (size_t si = 0; si < g->segs.size(); si++) {
     pb_segment_s* s = g->segs[si];
@@ -899,6 +901,10 @@ static int build_remaps(pb_group_s* g, const char* column, GlobalDict& gd) {
         return fail(PB_ERR_INVALID, "global dictionary of %s misses a value of segment %s", column, s->name.c_str());
       rm[i] = (int32_t)pos;
     }
+    // table-wide dimension dictionaries make most remaps the identity: a dependent load per key per doc saved
+    bool id = true;
+    for (int i = 0; i < c.card && id; i++) id = rm[i] == i;
+    gd.identity[si] = id ? 1 : 0;
   }
   return PB_OK;
 }
@@ -1002,7 +1008,8 @@ struct TableMeta {
 };
 
 // The aggregation kernel of a plan (AGG_NONE: the call has no docs, nothing to aggregate)
-enum AggKernel { AGG_NONE, AGG_GENERAL, AGG_SMEM, AGG_ROWS };   // pb_agg_kernel<6>, pb_agg_smem_kernel, pb_agg_rows_kernel
+// AGG_FUSED: the fused specialised filter kernel aggregates its own survivors, no aggregation kernel runs (plan_fused_agg)
+enum AggKernel { AGG_NONE, AGG_GENERAL, AGG_SMEM, AGG_ROWS, AGG_FUSED };   // pb_agg_kernel<6>, pb_agg_smem_kernel, pb_agg_rows_kernel
 
 struct pb_result_s {
   pb_group_s* group = nullptr;
@@ -1046,7 +1053,7 @@ struct pb_result_s {
     const DevExpandItem* expand_items = nullptr; int n_expand = 0;
     int U = 2; bool u2_three = false; size_t smem_filter = 0;
     int spec_w = 0, spec_pk = 0;             // > 0: the plan-time specialised filter kernel of that width / predicate kind
-    const DevRowSeg* row_segs = nullptr; int rows_rw = 0;   // AGG_ROWS: pb_agg_rows_kernel<rows_rw>
+    const DevRowSeg* row_segs = nullptr; int rows_rw = 0;   // AGG_ROWS: pb_agg_rows_kernel<rows_rw>; AGG_FUSED: the filter kernel's RW
     AggKernel agg = AGG_NONE;
     size_t smem_agg = 0;
     const DevLaneWeights* lane_w = nullptr; int n_lanes = 0, n_segs = 0;
@@ -1533,7 +1540,7 @@ static int enqueue_all(pb_result_s* r, const std::vector<cudaEvent_t>* seg_wait)
     if (seg_wait && rp.waves.size() > 1)
       for (int si = w.seg_lo; si < w.seg_hi; si++) if ((*seg_wait)[si]) CU(cudaStreamWaitEvent(st, (*seg_wait)[si], 0));
     if (w.grid_filter > 0 && rp.spec_w > 0) {
-      CU(pb_filter_spec_launch(rp.spec_w, rp.spec_pk, w.grid_filter, rp.smem_filter, st, &w.dq));
+      CU(pb_filter_spec_launch(rp.spec_w, rp.spec_pk, rp.agg == AGG_FUSED ? rp.rows_rw : 0, w.grid_filter, rp.smem_filter, st, &w.dq));
       r->launches++;
     } else if (w.grid_filter > 0) {
       if (rp.U == 1) pb_filter_kernel<1, 3><<<w.grid_filter, PB_NTHREADS, rp.smem_filter, st>>>(w.dq);
@@ -1686,7 +1693,6 @@ struct Plan {
   uint64_t n_chunks = 0, n_docs_total = 0;
   bool match_all = true;
   size_t st_rep_bytes = 0; int st_replicas = 0;     // CTA-private shared-memory table (pb_agg_smem_kernel)
-  uint32_t* d_match_list = nullptr;
   const unsigned long long* d_head = nullptr;
   const DevLaneWeights* d_lane_w = nullptr;
   const DevExpandItem* d_expand_items = nullptr;
@@ -2312,7 +2318,7 @@ static int bind_segment(Plan& P, int si) {
     kc.fwd = src.fwd; kc.n_full_words = src.full_words; kc.tail_word = src.tail_word;
     kc.bits = c.bits; kc.raw_width = c.has_dict ? 0 : c.raw_width; kc.data_type = c.type;
     kc.stride_bits = src.stride_bits; kc.bit_off = src.bit_off;
-    kc.remap = (P.combine && P.gdict[j]) ? P.gdict[j]->d_remap[si] : nullptr;
+    kc.remap = (P.combine && P.gdict[j] && !P.gdict[j]->identity[si]) ? P.gdict[j]->d_remap[si] : nullptr;
     kc.shift = tm.shifts[j];
     kc.mult = mult;
     if (tm.cards[j] > 0) mult *= (uint64_t)tm.cards[j];
@@ -2329,7 +2335,7 @@ static int bind_segment(Plan& P, int si) {
     ac.fwd = src.fwd; ac.n_full_words = src.full_words; ac.tail_word = src.tail_word;
     ac.dict_f64 = c.d_dict_f64; ac.bits = c.bits; ac.raw_width = fv >= 0 ? c.entry_bytes : c.has_dict ? 0 : c.raw_width; ac.data_type = c.type;
     ac.stride_bits = src.stride_bits; ac.bit_off = src.bit_off;
-    ac.remap = (P.combine && P.adict[a]) ? P.adict[a]->d_remap[si] : nullptr;
+    ac.remap = (P.combine && P.adict[a] && !P.adict[a]->identity[si]) ? P.adict[a]->d_remap[si] : nullptr;
   }
   return PB_OK;
 }
@@ -2437,8 +2443,7 @@ static int plan_units(Plan& P) {
 // How the matches reach the group table (see pb_device.cuh):
 //   smem      one dense table that fits shared memory and enough matches to amortise merging one private copy per CTA
 //   global    everything else: pb_agg_kernel, one thread per match, reductions straight into the global table
-// (rows: pb_agg_rows_kernel, see plan_rows_kernel).  A third way -- the filter kernel aggregating its own matches, no
-// match list -- was measured and removed: the two kernels are bound by the same memory system and did not overlap.
+// (rows: pb_agg_rows_kernel, see plan_rows_kernel; fused: the filter kernel aggregates its own survivors, see plan_fused_agg)
 static int plan_match_path(Plan& P) {
   pb_result_s* r = P.r;
   int n_acc = 0, n_fc = 0;
@@ -2453,11 +2458,17 @@ static int plan_match_path(Plan& P) {
     P.st_rep_bytes = pb_smem_table_bytes((uint32_t)r->tables[0].capacity, n_fc, n_acc);
     if (P.st_rep_bytes <= smem_table_budget) { P.st_replicas = 1; while (P.st_replicas < 32 && (size_t)(2 * P.st_replicas) * P.st_rep_bytes <= smem_table_budget) P.st_replicas *= 2; }
   }
-  if (!P.match_all && P.n_docs_total > 0) {
-    r->scratch = scratch_alloc(P.ctx, 4 * (size_t)P.n_docs_total + 256, &r->scratch_cap);
-    if (!r->scratch) return fail(PB_ERR_OOM, "match list allocation (%zu bytes) failed", 4 * (size_t)P.n_docs_total + 256);
-    P.d_match_list = (uint32_t*)r->scratch;
-  }
+  return PB_OK;
+}
+
+// The match list, once the launches are planned (a fused filter kernel writes none), and each wave's part of it
+static int alloc_match_list(Plan& P) {
+  pb_result_s* r = P.r;
+  if (P.match_all || P.n_docs_total == 0 || r->rp.agg == AGG_FUSED) return PB_OK;
+  r->scratch = scratch_alloc(P.ctx, 4 * (size_t)P.n_docs_total + 256, &r->scratch_cap);
+  if (!r->scratch) return fail(PB_ERR_OOM, "match list allocation (%zu bytes) failed", 4 * (size_t)P.n_docs_total + 256);
+  uint32_t* list = P.hq->match_list = (uint32_t*)r->scratch;
+  for (auto& w : r->rp.waves) w.dq.match_list = list + P.hsegs[w.seg_lo].doc_base;
   return PB_OK;
 }
 
@@ -2548,7 +2559,6 @@ static void fill_query(Plan& P) {
   hq->n_units = P.n_chunks; hq->segs = P.d_segs; hq->tables = P.d_tabs;
   hq->n_docs_total = P.n_docs_total; hq->match_all = P.match_all ? 1 : 0;
   { static const int sm = []() { const char* e = getenv("PB_SPARSE_MAX"); return e ? atoi(e) : PB_SPARSE_MAX; }(); hq->sparse_max = sm; }
-  hq->match_list = P.d_match_list;
   if (P.st_replicas > 0) {
     hq->st_slots = (int32_t)r->tables[0].capacity; hq->st_replicas = P.st_replicas;
     // merging a CTA's private table costs up to one RED per slot and aggregate: it pays once a CTA sees several matches per slot
@@ -2584,7 +2594,6 @@ static int plan_waves(Plan& P) {
       w.dq.unit_lo = P.hsegs[lo].unit_begin;
       w.dq.n_units = P.hsegs[hi - 1].unit_begin + P.hsegs[hi - 1].n_units - w.dq.unit_lo;
       w.dq.n_docs_total = P.hsegs[hi - 1].doc_base + (uint64_t)P.g->segs[hi - 1]->num_docs - P.hsegs[lo].doc_base;
-      w.dq.match_list = P.d_match_list + P.hsegs[lo].doc_base;
       w.dq.match_count = P.hq->match_count + waves.size();
       w.n_units = w.dq.n_units; w.n_docs = w.dq.n_docs_total;
       waves.push_back(w);
@@ -2650,11 +2659,48 @@ static void plan_filter_spec(Plan& P, size_t& smem, uint64_t& max_ctas) {
   int oc = PB_OUT_CAP, cc = PB_CAND_CAP;
   if (4 * (filter_smem(P, PB_OUT_CAP / 2, PB_CAND_CAP / 2) + 1024) <= 227 * 1024 && 4 * (smem + 1024) > 227 * 1024) { oc /= 2; cc /= 2; smem_spec = filter_smem(P, oc, cc); }
   int occ = 0;
-  if (pb_filter_spec_prepare(w, pk, smem_spec, &occ) == cudaSuccess && occ >= 1) {
+  if (pb_filter_spec_prepare(w, pk, 0, smem_spec, &occ) == cudaSuccess && occ >= 1) {
     rp.spec_w = w; rp.spec_pk = pk; max_ctas = (uint64_t)P.ctx->num_sms * (uint64_t)occ; smem = smem_spec;
     P.hq->out_cap = oc; P.hq->cand_cap = cc; P.hq->cand_bytes = P.any_cand_leaf ? (int32_t)(2 * cc * PB_NWARPS) : 0;
     for (auto& wv : rp.waves) { wv.dq.out_cap = oc; wv.dq.cand_cap = cc; wv.dq.cand_bytes = P.hq->cand_bytes; }
   } else cudaGetLastError();
+}
+
+// Fused aggregation (pb_filter_kernel<2, 4, W, K, RW>): when every candidate leaf is a dictId field of the segment's row
+// group, the candidate round already reads each candidate's 32-byte row sector, so it loads the whole row once, tests the
+// leaves from registers and aggregates a survivor on the spot (field extraction + fire-and-forget REDs).  The match list
+// (written, flushed, read back, searched for its segment) and pb_agg_rows_kernel with its launch gap go away.  An earlier
+// fused path that buffered the matches and gathered every column in separate rounds at the end of each warp's range was
+// measured and removed: it added dependent DRAM round trips that did not overlap the streaming.  This one adds none.
+// Only where pb_agg_rows_kernel would update the global table anyway: expected matches below st_min_docs, one wave.
+// On success it takes over the filter launch (shared memory, CTAs per launch) and returns true.
+static bool plan_fused_agg(Plan& P, size_t& smem, uint64_t& max_ctas) {
+  static const bool fused_on = []() { const char* e = getenv("PB_FUSED_AGG"); return !e || atoi(e) != 0; }();
+  pb_result_s* r = P.r;
+  pb_result_s::Replay& rp = r->rp;
+  if (!(fused_on && rp.spec_w > 0 && P.any_cand_leaf && P.d_row_segs && !r->track_first && P.nF == 0 && r->table_mode == T_DENSE &&
+        rp.waves.size() == 1)) return false;
+  double expected = 0;
+  for (int si = 0; si < P.n_segs; si++) {
+    const DevSegQuery& ds = P.hsegs[si];
+    for (int n = 0; n < ds.n_nodes; n++) {
+      if (ds.node_kind[n] != N_LEAF) continue;
+      const DevLeaf& lf = ds.leaves[ds.node_arg[n]];
+      const bool row_field = (lf.kind == L_DICT_RANGE || lf.kind == L_DICT_SET) && (const void*)lf.gfwd == (const void*)P.h_row_segs[si].rows &&
+                             lf.g_stride_bits == 32 * P.rows_rw;
+      if (lf.gather && !row_field) return false;
+    }
+    expected += estimate_selectivity(P.g->segs[si], P.sqs[si]) * (double)P.g->segs[si]->num_docs;
+  }
+  if (P.st_replicas > 0 && expected >= (double)P.hq->st_min_docs) return false;
+  // no output buffer; the segment's DevRowSeg sits behind the header
+  const size_t smem_fused = filter_smem(P, 0, P.hq->cand_cap) + ((sizeof(DevRowSeg) + 127) & ~(size_t)127);
+  int occ = 0;
+  if (pb_filter_spec_prepare(rp.spec_w, rp.spec_pk, P.rows_rw, smem_fused, &occ) != cudaSuccess || occ < 1) { cudaGetLastError(); return false; }
+  smem = smem_fused; max_ctas = (uint64_t)P.ctx->num_sms * (uint64_t)occ;
+  P.hq->out_cap = 0; P.hq->row_segs = P.d_row_segs;
+  for (auto& wv : rp.waves) { wv.dq.out_cap = 0; wv.dq.row_segs = P.d_row_segs; }
+  return true;
 }
 
 // Kernel choice and launch geometry of the call, saved in r->rp so that a cached plan can enqueue them again
@@ -2696,6 +2742,7 @@ static int plan_launches(Plan& P) {
     max_ctas = (uint64_t)ctx->num_sms * (uint64_t)occ;
   }
   plan_filter_spec(P, smem, max_ctas);
+  const bool fused = plan_fused_agg(P, smem, max_ctas);
   rp.smem_filter = smem;
   const bool use_smem_table = P.st_replicas > 0;
   const size_t smem2 = r->table_mode == T_KEYLESS ? (P.nF > 0 ? 3 : 2) * sizeof(double) * (size_t)P.nA * PB_NTHREADS : 0;
@@ -2708,7 +2755,7 @@ static int plan_launches(Plan& P) {
     max2 = (uint64_t)ctx->num_sms * (uint64_t)occ2;
   }
   rp.expand_items = P.d_expand_items; rp.n_expand = (int)P.expand_items.size();
-  rp.agg = P.n_docs_total == 0 ? AGG_NONE : P.d_row_segs ? AGG_ROWS : use_smem_table ? AGG_SMEM : AGG_GENERAL;
+  rp.agg = P.n_docs_total == 0 ? AGG_NONE : fused ? AGG_FUSED : P.d_row_segs ? AGG_ROWS : use_smem_table ? AGG_SMEM : AGG_GENERAL;
   const bool smem_threads = rp.agg == AGG_SMEM || rp.agg == AGG_ROWS;   // PB_AGG_SMEM_THREADS per CTA, one CTA per SM
   rp.smem_agg = (use_smem_table && smem_threads) ? (size_t)P.st_replicas * P.st_rep_bytes : rp.agg == AGG_ROWS ? 0 : smem2;
   rp.row_segs = P.d_row_segs; rp.rows_rw = P.rows_rw;
@@ -2716,7 +2763,7 @@ static int plan_launches(Plan& P) {
   for (auto& wl : rp.waves) {
     // every CTA gets a contiguous range of chunks; keep at least one chunk per warp
     wl.grid_filter = (!P.match_all && wl.n_units > 0) ? (int)std::min<uint64_t>(std::max<uint64_t>((wl.n_units + PB_NWARPS - 1) / PB_NWARPS, 1), max_ctas) : 0;
-    if (wl.n_docs == 0 || rp.agg == AGG_NONE) wl.grid_agg = 0;
+    if (wl.n_docs == 0 || rp.agg == AGG_NONE || rp.agg == AGG_FUSED) wl.grid_agg = 0;
     else if (smem_threads) wl.grid_agg = (int)std::min<uint64_t>(std::max<uint64_t>((wl.n_docs + PB_AGG_SMEM_THREADS - 1) / PB_AGG_SMEM_THREADS, 1), (uint64_t)ctx->num_sms);
     else wl.grid_agg = (int)std::min<uint64_t>(std::max<uint64_t>((wl.n_docs + PB_NTHREADS - 1) / PB_NTHREADS, 1), max2);
   }
@@ -2726,15 +2773,18 @@ static int plan_launches(Plan& P) {
   for (auto& tm : r->tables) if (tm.capacity + 1 > (1ull << 20)) small = false;
   rp.cacheable = P.n_pending == 0 && !P.in_place && rp.waves.size() == 1 && small && !(P.q->flags & PB_Q_DEFER_FINALIZE) && r->in_place_columns == 0;
   int32_t* pi = r->plan_info;
-  pi[0] = (int32_t)rp.agg; pi[1] = rp.agg == AGG_ROWS ? rp.rows_rw : 0;
-  pi[2] = P.st_replicas; pi[3] = P.st_replicas > 0 ? (int32_t)std::min<uint64_t>(P.hq->st_min_docs, INT32_MAX) : 0;
+  // a fused call reports the rows kernel's path it replaces: its row width, no CTA table
+  const int st_replicas = fused ? 0 : P.st_replicas;
+  pi[0] = (int32_t)(fused ? AGG_ROWS : rp.agg); pi[1] = (rp.agg == AGG_ROWS || fused) ? rp.rows_rw : 0;
+  pi[2] = st_replicas; pi[3] = st_replicas > 0 ? (int32_t)std::min<uint64_t>(P.hq->st_min_docs, INT32_MAX) : 0;
   pi[4] = r->table_mode; pi[5] = r->key_words;
   pi[6] = (P.match_all || P.n_chunks == 0) ? 0 : rp.spec_w > 0 ? 3 : rp.U;
   pi[7] = rp.spec_w; pi[8] = rp.spec_w > 0 ? rp.spec_pk : 0;
   pi[9] = P.any_cand_leaf ? 1 : 0;
   pi[10] = 0;
   // (the rows kernel sums exactly only in the CTA-private table: without one the flag is not used)
-  if (P.h_row_segs && P.st_replicas > 0) for (int a = 0; a < P.nA; a++) if (P.h_row_segs[0].aggs[a].exact_int) pi[10] |= 1 << a;
+  if (P.h_row_segs && st_replicas > 0) for (int a = 0; a < P.nA; a++) if (P.h_row_segs[0].aggs[a].exact_int) pi[10] |= 1 << a;
+  pi[11] = fused ? 1 : 0;
   return PB_OK;
 }
 
@@ -2788,7 +2838,7 @@ static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, c
   fill_query(P);
   if ((rc = put_expand_items(P)) || (rc = plan_waves(P)) || (rc = upload_descriptors(P))) return rc;
   lap(2);
-  if ((rc = plan_launches(P)) || (rc = enqueue_all(r, &P.seg_wait))) return rc;
+  if ((rc = plan_launches(P)) || (rc = alloc_match_list(P)) || (rc = enqueue_all(r, &P.seg_wait))) return rc;
   lap(3);
 
   if (q->flags & PB_Q_DEFER_FINALIZE) {

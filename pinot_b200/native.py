@@ -25,9 +25,10 @@ PB_Q_GATHER_IN_PLACE = 16
 PB_Q_ALL_RANKS = 32
 PB_COMM_ID_BYTES = 128
 # pb_result_plan_info, in order.  agg_kernel: 0 none, 1 general, 2 smem table, 3 rows; table_mode: 0 keyless, 1 dense,
-# 2 hash; filter_kernel: 0 none, 1 general U=1, 2 general U=2, 3 specialised (spec_w, spec_k)
+# 2 hash; filter_kernel: 0 none, 1 general U=1, 2 general U=2, 3 specialised (spec_w, spec_k); fused_agg: 1 when the
+# specialised filter kernel aggregates its own survivors (agg_kernel 3 and rows_rw then name the path it replaces)
 PLAN_INFO_FIELDS = ("agg_kernel", "rows_rw", "st_replicas", "st_min_docs", "table_mode", "key_words", "filter_kernel",
-                    "spec_w", "spec_k", "cand_leaf", "exact_int_mask")
+                    "spec_w", "spec_k", "cand_leaf", "exact_int_mask", "fused_agg")
 
 
 class PbColumnDesc(C.Structure):
