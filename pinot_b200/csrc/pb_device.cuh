@@ -158,6 +158,7 @@ struct DevTable {
   uint64_t dset_mask[PB_MAX_AGGS];
   unsigned long long* dcnt[PB_MAX_AGGS];
   unsigned int* num_groups;          // hash: groups created so far
+  unsigned int* sentinel_claim;      // hash: 1 once the all-ones key holds a ticket for its reserved slot
   unsigned int* limit_reached;
   unsigned int* any_limit;           // query-wide: some hash table of this launch refused a key (drives the repair pass)
   unsigned long long* docs_matched;  // numDocsScanned
@@ -540,7 +541,9 @@ __device__ __forceinline__ uint64_t pb_hash64(uint64_t k) {
 // reference's "existing groups keep aggregating, new keys are ignored". ----
 __device__ __forceinline__ bool pb_group_ticket(const DevTable& t) {
   if (!t.limit_active) return true;                      // groups <= docs <= limit: cannot be reached, nothing to count
-  const unsigned m = __activemask();
+  // one draw per table among the active lanes: a warp of a per-segment call can hold docs of two segments, whose tables
+  // count their groups apart
+  const unsigned m = __match_any_sync(__activemask(), (unsigned long long)t.num_groups);
   const int leader = __ffs(m) - 1, lane = (int)(threadIdx.x & 31);
   const unsigned rank = __popc(m & ((1u << lane) - 1u)), need = __popc(m);
   unsigned base = 0;
@@ -552,10 +555,19 @@ __device__ __forceinline__ bool pb_group_ticket(const DevTable& t) {
   return false;
 }
 __device__ __forceinline__ void pb_group_ticket_return(const DevTable&) {}
+// The all-ones key has a reserved slot (t.capacity) instead of a claim in the key array; under a reachable limit its
+// first insert takes a ticket like any other new key.  (Racing first inserts may each take one: a lost ticket, as above.)
+__device__ __forceinline__ uint64_t pb_sentinel_slot(const DevTable& t, bool insert) {
+  if (!t.limit_active) return t.capacity;
+  if (*(volatile unsigned int*)t.sentinel_claim) return t.capacity;
+  if (!insert || !pb_group_ticket(t)) return ~0ull;
+  atomicExch(t.sentinel_claim, 1u);
+  return t.capacity;
+}
 
 // returns slot, or ~0ull when the key is new and numGroupsLimit is reached
 __device__ __forceinline__ uint64_t pb_hash_slot(const DevTable& t, uint64_t key, bool insert = true) {
-  if (key == PB_HASH_EMPTY) return t.capacity;          // reserved extra slot for the sentinel value itself
+  if (key == PB_HASH_EMPTY) return pb_sentinel_slot(t, insert);   // reserved extra slot for the sentinel value itself
   uint64_t mask = t.capacity - 1;
   uint64_t s = pb_hash64(key) & mask;
   for (uint64_t probes = 0; probes <= mask; probes++) {
@@ -583,7 +595,7 @@ __device__ __forceinline__ void pb_atom_cas_u128(unsigned long long* p, unsigned
                : "=l"(olo), "=l"(ohi) : "l"(clo), "l"(chi), "l"(vlo), "l"(vhi), "l"(p) : "memory");
 }
 __device__ __forceinline__ uint64_t pb_hash_slot2(const DevTable& t, uint64_t lo, uint64_t hi, bool insert = true) {
-  if (lo == PB_HASH_EMPTY && hi == PB_HASH_EMPTY) return t.capacity;     // reserved slot for the sentinel pattern itself
+  if (lo == PB_HASH_EMPTY && hi == PB_HASH_EMPTY) return pb_sentinel_slot(t, insert);     // reserved slot for the sentinel pattern itself
   const uint64_t mask = t.capacity - 1;
   uint64_t s = pb_hash64(lo ^ pb_hash64(hi)) & mask;
   for (uint64_t probes = 0; probes <= mask; probes++) {
@@ -1448,10 +1460,12 @@ __global__ void __launch_bounds__(PB_NTHREADS, MIN_CTAS) pb_agg_kernel(const __g
     uint32_t fpass = 0;
     if (nF > 0) {
       fpass = pb_agg_filter_bits(sg, doc);
-      if (lo != stat_seg) { stat_flush(); stat_seg = lo; }
-      stat_cnt[0]++;
+      if (Q.phase != 2) {           // (the repair pass reads the same matches again: their lanes were counted)
+        if (lo != stat_seg) { stat_flush(); stat_seg = lo; }
+        stat_cnt[0]++;
 #pragma unroll
-      for (int f = 0; f < PB_MAX_AGG_FILTERS; f++) if (f < nF) stat_cnt[1 + f] += (fpass >> f) & 1u;
+        for (int f = 0; f < PB_MAX_AGG_FILTERS; f++) if (f < nF) stat_cnt[1 + f] += (fpass >> f) & 1u;
+      }
     }
     pb_accumulate(Q, sg, Q.tables[table], doc, ka, keyless_rows, fpass);
   }
@@ -2082,7 +2096,11 @@ struct DevOrderKey {
   const unsigned long long* fcnt;
   unsigned long long* okey;
 };
+// a double in Double.compare order (the order TableResizer sorts final results in): -0.0 < 0.0, and every NaN is one value
+// above +inf
+__device__ __forceinline__ long long pb_order_f64(double v) { return isnan(v) ? 0x7ff8000000000000LL : pb_enc_f64(v); }
 static __global__ void pb_order_key_kernel(const DevOrderKey K) {
+  const double inf = __longlong_as_double(0x7ff0000000000000LL);
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < K.S; i += (uint64_t)gridDim.x * blockDim.x) {
     const unsigned long long c = K.rowcnt[i];
     unsigned long long u = 0;
@@ -2090,8 +2108,14 @@ static __global__ void pb_order_key_kernel(const DevOrderKey K) {
       if (K.kind == 1) {
         long long e;
         if (K.op == 0) e = (long long)(K.fcnt ? K.fcnt[i] : c);                                        // COUNT
-        else if (K.op == 1) e = pb_enc_f64(K.sum[i]);                                                   // SUM
-        else if (K.op == 4) { const unsigned long long n = K.fcnt ? K.fcnt[i] : c; e = pb_enc_f64(n ? K.sum[i] / (double)n : 0.0); }   // AVG
+        else if (K.op == 1) e = pb_order_f64(K.sum[i]);                                                 // SUM
+        else if (K.op == 4) {                                                                           // AVG
+          // no input (a FILTER clause left the group nothing): AvgAggregationFunction.extractFinalResult gives
+          // DEFAULT_FINAL_RESULT = Double.NEGATIVE_INFINITY, below every real average
+          const unsigned long long n = K.fcnt ? K.fcnt[i] : c;
+          e = pb_order_f64(n ? K.sum[i] / (double)n : -inf);
+        }
+        else if (K.mm[i] == 0x7fffffffffffffffLL) e = pb_enc_f64(K.op == 2 ? inf : -inf);              // MIN / MAX without input: the +-inf the hand-back emits
         else e = K.op == 2 ? K.mm[i] : ~K.mm[i];                                                        // MIN / MAX (encoded; MAX is stored complemented)
         u = (unsigned long long)e ^ 0x8000000000000000ull;
       } else {
@@ -2105,7 +2129,7 @@ static __global__ void pb_order_key_kernel(const DevOrderKey K) {
           else field = khi >> (K.shift - 64);
           if (K.width < 64) field &= ((1ull << K.width) - 1ull);
         }
-        if (K.field_is_double) u = (unsigned long long)pb_enc_f64(__longlong_as_double((long long)field)) ^ 0x8000000000000000ull;
+        if (K.field_is_double) u = (unsigned long long)pb_order_f64(__longlong_as_double((long long)field)) ^ 0x8000000000000000ull;
         else if (K.field_is_signed) u = (K.width == 32 ? (unsigned long long)(long long)(int32_t)(uint32_t)field : field) ^ 0x8000000000000000ull;
         else u = field;                                                                                  // dictId: sorted dictionary order
       }
@@ -2114,18 +2138,21 @@ static __global__ void pb_order_key_kernel(const DevOrderKey K) {
     K.okey[i] = u;
   }
 }
-// radix select, one 8-bit digit per pass: state = {prefix, k remaining, done, threshold, candidates}
+// radix select, one 8-bit digit per pass: state = {prefix, k remaining, done, threshold, candidates}.  The candidates are the
+// groups the numGroupsLimit cut keeps (first_doc[slot] <= *first_thr, when the table tracks first docs): Pinot limits the
+// keys in the key generator and trims what is left.
 struct DevSelectState { unsigned long long prefix, k, done, thr, total; unsigned long long hist[256]; };
 static __global__ void pb_rselect_hist_kernel(const unsigned long long* __restrict__ okey, const unsigned long long* __restrict__ rowcnt, uint64_t S, int pass,
-                                              DevSelectState* st) {
+                                              const uint32_t* __restrict__ first_doc, const uint32_t* __restrict__ first_thr, DevSelectState* st) {
   __shared__ unsigned int h[256];
   for (int b = threadIdx.x; b < 256; b += blockDim.x) h[b] = 0;
   __syncthreads();
   if (!st->done) {
     const unsigned long long prefix = st->prefix;
     const unsigned long long hi_mask = pass == 7 ? 0ull : (~0ull << (8 * (pass + 1)));
+    const uint32_t fthr = first_doc ? *first_thr : 0u;
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < S; i += (uint64_t)gridDim.x * blockDim.x) {
-      if (!rowcnt[i]) continue;
+      if (!rowcnt[i] || (first_doc && first_doc[i] > fthr)) continue;
       const unsigned long long v = okey[i];
       if ((v & hi_mask) == (prefix & hi_mask)) atomicAdd(&h[(v >> (8 * pass)) & 255u], 1u);
     }
@@ -2133,7 +2160,9 @@ static __global__ void pb_rselect_hist_kernel(const unsigned long long* __restri
   __syncthreads();
   for (int b = threadIdx.x; b < 256; b += blockDim.x) if (h[b]) atomicAdd(&st->hist[b], (unsigned long long)h[b]);
 }
-static __global__ void pb_rselect_pick_kernel(DevSelectState* st, int pass, unsigned long long trim_size, unsigned long long trim_threshold) {
+// (pass 7 also sets the numGroupsLimit flag from the group count before the trim: GroupByOperator.java:116)
+static __global__ void pb_rselect_pick_kernel(DevSelectState* st, int pass, unsigned long long trim_size, unsigned long long trim_threshold,
+                                              unsigned long long num_groups_limit, unsigned int* limit_reached) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   if (pass == 7) { st->prefix = 0; st->k = trim_size; st->done = 0; st->thr = 0; }
   if (!st->done) {
@@ -2141,6 +2170,7 @@ static __global__ void pb_rselect_pick_kernel(DevSelectState* st, int pass, unsi
       unsigned long long total = 0;
       for (int b = 0; b < 256; b++) total += st->hist[b];
       st->total = total;
+      if (total >= num_groups_limit) *limit_reached = 1u;
       if (total <= trim_threshold || total <= st->k) { st->done = 1; st->thr = 0; }      // the table is small enough: keep everything
     }
     if (!st->done) {
@@ -2154,12 +2184,15 @@ static __global__ void pb_rselect_pick_kernel(DevSelectState* st, int pass, unsi
   for (int b = 0; b < 256; b++) st->hist[b] = 0;
 }
 
-// count non-empty slots (that survive the ORDER BY trim, if any)
+// count non-empty slots (that survive the numGroupsLimit cut and the ORDER BY trim, if any)
 static __global__ void pb_count_groups_kernel(const unsigned long long* __restrict__ rowcnt, uint64_t n, unsigned long long* out,
+                                              const uint32_t* __restrict__ first_doc, const uint32_t* __restrict__ first_thr,
                                               const unsigned long long* __restrict__ okey, const unsigned long long* __restrict__ othr) {
   unsigned long long c = 0;
   const unsigned long long thr = othr ? *othr : 0ull;
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) c += rowcnt[i] != 0 && (!okey || okey[i] >= thr);
+  const uint32_t fthr = first_doc ? *first_thr : 0u;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    c += rowcnt[i] != 0 && (!first_doc || first_doc[i] <= fthr) && (!okey || okey[i] >= thr);
   for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }

@@ -2014,6 +2014,7 @@ static int lay_out_tables(Plan& P) {
     if (!P.d_zero) continue;
     unsigned long long* cnt = r->d_counters + (size_t)t * PB_COUNTERS_PER_TABLE;
     dt.num_groups = reinterpret_cast<unsigned int*>(cnt + 0);
+    dt.sentinel_claim = reinterpret_cast<unsigned int*>(cnt + 0) + 1;     // (the upper half of the group-count cell)
     dt.limit_reached = reinterpret_cast<unsigned int*>(cnt + 1);
     dt.any_limit = reinterpret_cast<unsigned int*>(P.d_aux + P.any_limit_off);
     dt.docs_matched = cnt + 2;
@@ -2584,7 +2585,8 @@ static int put_expand_items(Plan& P) {
 static int plan_waves(Plan& P) {
   std::vector<pb_result_s::WaveLaunch>& waves = P.r->rp.waves;
   const int n_segs = P.n_segs;
-  if (P.n_pending > 0 && !P.match_all && P.expand_items.empty() && n_segs > 1 && P.n_chunks > 0) {
+  // (a hash table under a reachable numGroupsLimit runs in one wave: its repair pass re-aggregates the whole call's matches)
+  if (P.n_pending > 0 && !P.match_all && P.expand_items.empty() && n_segs > 1 && P.n_chunks > 0 && !P.r->repair_pass) {
     const int per_wave = (n_segs + PB_MAX_WAVES - 1) / PB_MAX_WAVES;
     for (int lo = 0; lo < n_segs; lo += per_wave) {
       const int hi = std::min(n_segs, lo + per_wave);
@@ -2972,10 +2974,19 @@ extern "C" int pb_query_execute(pb_segment_group_handle g, const pb_segment_quer
 // finalize: compaction of non-empty groups, device -> pinned host, key decode
 // ------------------------------------------------------------------------------------------------
 
-// ORDER BY ... LIMIT trim: order keys of every table + the grid-wide radix select of the trim_size-th best (8 digit passes)
+// The groups a table hands back: first the numGroupsLimit cut in doc order (dense tables that track first docs), then the
+// ORDER BY ... LIMIT trim over the groups the cut keeps -- order keys of every table + the grid-wide radix select of the
+// trim_size-th best (8 digit passes).  Pinot limits the keys in the key generator and trims what is left.
 static int enqueue_trim(pb_result_s* r) {
-  if (r->trim_size <= 0 || r->table_mode == T_KEYLESS) return PB_OK;
   cudaStream_t st = r->stream;
+  for (size_t t = 0; t < r->tables.size(); t++) {
+    const DevTable& dt = r->tables[t].dev;
+    if (!dt.first_doc) continue;
+    pb_select_first_kernel<<<1, 1024, 0, st>>>(dt.first_doc, r->tables[t].capacity, dt.num_groups_limit, r->d_first_thr + t);
+    r->launches++;
+  }
+  CU(cudaGetLastError());
+  if (r->trim_size <= 0 || r->table_mode == T_KEYLESS) return PB_OK;
   pb_group_s* g = r->group;
   for (size_t t = 0; t < r->tables.size(); t++) {
     TableMeta& tm = r->tables[t];
@@ -2997,9 +3008,11 @@ static int enqueue_trim(pb_result_s* r) {
     }
     const int grid = (int)std::min<uint64_t>((K.S + 255) / 256, (uint64_t)r->ctx->num_sms * 8);
     pb_order_key_kernel<<<grid, 256, 0, st>>>(K);
+    const uint32_t* first_thr = tm.dev.first_doc ? r->d_first_thr + t : nullptr;
     for (int pass = 7; pass >= 0; pass--) {
-      pb_rselect_hist_kernel<<<grid, 256, 0, st>>>(K.okey, K.rowcnt, K.S, pass, r->d_sel[t]);
-      pb_rselect_pick_kernel<<<1, 32, 0, st>>>(r->d_sel[t], pass, (unsigned long long)r->trim_size, (unsigned long long)r->trim_threshold);
+      pb_rselect_hist_kernel<<<grid, 256, 0, st>>>(K.okey, K.rowcnt, K.S, pass, tm.dev.first_doc, first_thr, r->d_sel[t]);
+      pb_rselect_pick_kernel<<<1, 32, 0, st>>>(r->d_sel[t], pass, (unsigned long long)r->trim_size, (unsigned long long)r->trim_threshold,
+                                               (unsigned long long)tm.dev.num_groups_limit, tm.dev.limit_reached);
     }
     r->launches += 17;
   }
@@ -3029,6 +3042,7 @@ static int prepare_finalize(pb_result_s* r) {
       any_big = true;
       int grid = (int)std::min<uint64_t>((S + 255) / 256, 2048);
       pb_count_groups_kernel<<<grid, 256, 0, st>>>(tm.dev.rowcnt, S, r->d_counters + (size_t)t * PB_COUNTERS_PER_TABLE + 3,
+                                                   tm.dev.first_doc, tm.dev.first_doc ? r->d_first_thr + t : nullptr,
                                                    r->trim_size > 0 ? r->d_okey[(size_t)t] : nullptr, r->trim_size > 0 ? &r->d_sel[(size_t)t]->thr : nullptr);
       r->launches++;
     }
@@ -3110,10 +3124,6 @@ static int enqueue_finalize(pb_result_s* r) {
       pb_dset_count_kernel<<<(int)std::min<uint64_t>((cap + 255) / 256, (uint64_t)r->ctx->num_sms * 8), 256, 0, st>>>(dt.dset[a], cap, dt.dcnt[a]);
       r->launches++;
     }
-    if (F.first_doc) {
-      pb_select_first_kernel<<<1, 1024, 0, st>>>(F.first_doc, F.S, r->tables[(size_t)t].dev.num_groups_limit, r->d_first_thr + t);
-      r->launches++;
-    }
     pb_finalize_kernel<<<r->rp.fin_grid[(size_t)t], 256, 0, st>>>(F);
     r->launches++;
   }
@@ -3183,6 +3193,8 @@ static int finish_finalize(pb_result_s* r) {
       return fail(PB_ERR_STATE, "cross-GPU merge: table layouts differ across ranks (different query or global dictionaries)");
     tm.stats.num_groups_limit_reached = 0;
     if (nG > 0) {
+      // (the flag cell also holds the trim's verdict on the group count before the trim, pb_rselect_pick_kernel: ng counts
+      //  the groups emitted, which a trim may have cut below the limit)
       bool flag = (uint32_t)hc[(size_t)t * PB_COUNTERS_PER_TABLE + 1] != 0;
       tm.stats.num_groups_limit_reached = (flag || ng >= (int64_t)tm.dev.num_groups_limit) ? 1 : 0;   // GroupByOperator.java:116
     }

@@ -377,9 +377,16 @@ def parse_sql(sql: str) -> QueryContext:
                 else:
                     col = p.ident()
                 p.eat_op(")")
-                hits = [i for i, a in enumerate(aggs) if a.op == op and a.column == col and a.filter is None]
+                ob_filter = None
+                if p.kw("FILTER"):          # names the SELECT-list entry with the identical FILTER clause
+                    p.i += 1
+                    p.eat_op("(")
+                    p.eat_kw("WHERE")
+                    ob_filter = p.or_expr()
+                    p.eat_op(")")
+                hits = [i for i, a in enumerate(aggs) if a.op == op and a.column == col and a.filter == ob_filter]
                 if not hits:
-                    raise ValueError(f"ORDER BY {name}({col or '*'}) is not in the SELECT list")
+                    raise ValueError(f"ORDER BY {name}({col or '*'}){' FILTER(...)' if ob_filter is not None else ''} is not in the SELECT list")
                 ob = (1, hits[0])
             else:
                 if name not in group_by:

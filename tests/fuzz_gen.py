@@ -195,3 +195,28 @@ def make_query(rng, src: Dict[str, Col]) -> str:
         aggs.append(f"{op}({col}){flt}")
     gb = f" GROUP BY {', '.join(keys)} LIMIT 100000000" if keys else ""
     return f"SET numGroupsLimit = 100000000; SELECT {', '.join(aggs)} FROM t{where_clause(rng, src)}{gb}"
+
+
+def make_shaped_query(rng, src: Dict[str, Col]) -> str:
+    """A group-by query whose result is shaped on the device: ORDER BY a key column or a (possibly filtered) non-DISTINCTCOUNT
+    aggregation, ASC or DESC, LIMIT 1-4 and trim sizes small enough that the trim fires on tables above ~10 groups (and
+    stays off on k3 and k2, k3); for about half the queries a numGroupsLimit below the key space.  Its own rng stream
+    (make_query's seeds and coverage stay as they are)."""
+    keys = KEY_SETS[int(rng.integers(1, len(KEY_SETS)))]
+    aggs = []
+    for _ in range(int(rng.integers(1, 5))):
+        op = str(rng.choice(["COUNT", "SUM", "MIN", "MAX", "AVG"]))
+        col = "*" if op == "COUNT" else str(rng.choice(MINMAX_COLS if op in ("MIN", "MAX") else SUM_COLS))
+        flt = f" FILTER(WHERE {_expr(rng, src, 1)})" if rng.random() < 0.3 else ""
+        aggs.append(f"{op}({col}){flt}")
+    if rng.random() < 0.4:
+        ob = str(rng.choice(keys))
+    else:
+        ob = aggs[int(rng.integers(0, len(aggs)))]
+    limit = int(rng.integers(1, 5))
+    size = int(rng.integers(6, 11))             # (5 x LIMIT is at most 20)
+    opts = f"SET minServerGroupTrimSize = {size}; SET minSegmentGroupTrimSize = {size}; " \
+           f"SET groupTrimThreshold = {int(rng.integers(1, 3)) * max(size, 5 * limit)}; "
+    ngl = int(rng.choice([1, 2, 5, 20, 300])) if rng.random() < 0.5 else 100000000
+    return f"SET numGroupsLimit = {ngl}; {opts}SELECT {', '.join(aggs)} FROM t{where_clause(rng, src)} GROUP BY {', '.join(keys)} " \
+           f"ORDER BY {ob} {'DESC' if rng.random() < 0.5 else 'ASC'} LIMIT {limit}"

@@ -162,9 +162,11 @@ def _key_of(c: Col, x):
     return float(x)
 
 
-def reference(table, q) -> Dict[tuple, list]:
+def reference(table, q, first_groups: Optional[int] = None) -> Dict[tuple, list]:
     """key -> per aggregation: COUNT int, SUM / AVG SumRef, MIN / MAX float, DISTINCTCOUNT int.  Every group the main
-    filter leaves docs in exists (FILTER clauses do not create or remove groups); keyless: the one row () always."""
+    filter leaves docs in exists (FILTER clauses do not create or remove groups); keyless: the one row () always.
+    first_groups: keep only the groups of the first that many distinct keys in doc order among the docs the main filter
+    keeps, with their full aggregates (a key generator that creates groups first come first served)."""
     table = _table(table)
     n = _num_docs(table)
     main = evaluate_sql(table, q.filter)
@@ -239,7 +241,144 @@ def reference(table, q) -> Dict[tuple, list]:
                     vals.append(SumRef(ex, int(cnt[i]), float(abs_sum[i]), float(max_abs[i]), False))
         for k, v in zip(group_keys, vals):
             out[k].append(v)
+    if first_groups is not None and keys:
+        admitted = np.argsort(first, kind="stable")[:first_groups]
+        out = {group_keys[g]: out[group_keys[g]] for g in admitted}
     return out
+
+
+# ---- numGroupsLimit ----
+
+class LimitRef(NamedTuple):
+    rows: Dict[tuple, list]      # exact: the groups the device hands back; else a superset of them
+    exact: bool
+    at_most: int                 # the device hands back at most this many groups
+    reached: Optional[bool]      # the num_groups_limit_reached the device must report (None: either)
+
+
+def limit_reference(table, q, mode: str, key_space: int = 0) -> LimitRef:
+    """What a table under q.num_groups_limit hands back (before any ORDER BY trim), DESIGN.md §4.5.  The flag follows
+    GroupByOperator.java:116: the key generator's group count (at most the limit) reached the limit.
+    mode 'dense': a dense per-segment table, or a combined call over one segment; key_space = the product of the segment's
+      dictionary cardinalities of the key columns.  Below it the key generator creates groups first come first served
+      (IntMapBasedHolder, DictionaryBasedGroupKeyGenerator.java:1023-1058): the first `limit` keys in doc order, complete.
+    mode 'merged': a dense table over several segments merged on the device: every group (a superset of what Pinot keeps).
+    mode 'hash': the limit in thread order -- at most `limit` groups, each complete; when there are at least `limit` groups
+      the flag is set.  (A ticket lost to a racing claim may refuse a key below the limit: then the flag is set too, so a
+      result without the flag holds every group.)"""
+    limit = max(1, q.num_groups_limit)
+    full = reference(table, q)
+    n = len(full) if q.group_by else 0
+    if mode == "dense" and limit < key_space:
+        return LimitRef(reference(table, q, first_groups=limit), True, limit, n >= limit)
+    if mode == "hash":
+        return LimitRef(full, False, limit, True if n >= limit else None)
+    return LimitRef(full, True, max(n, 1), n >= limit)
+
+
+def assert_limit_matches(got_rows: Dict[tuple, list], got_reached: int, lref: LimitRef, q, what=""):
+    """the group set and the flag against limit_reference (before any trim), every returned group complete"""
+    assert got_reached in (0, 1) and (lref.reached is None or bool(got_reached) == lref.reached), \
+        f"{what}: num_groups_limit_reached {got_reached}, expected {int(lref.reached)}"
+    assert len(got_rows) <= lref.at_most, f"{what}: {len(got_rows)} groups > {lref.at_most}"
+    if lref.exact or not got_reached:
+        assert_matches_reference(got_rows, lref.rows, q, what)
+    else:
+        extra = [k for k in got_rows if k not in lref.rows]
+        assert not extra, f"{what}: groups not in the reference: {extra[:3]}"
+        assert_matches_reference(got_rows, {k: lref.rows[k] for k in got_rows}, q, what)
+
+
+# ---- the ORDER BY ... LIMIT trim ----
+# TableResizer orders the groups by the first ORDER BY expression: a group-by column by its value, an aggregation by its
+# final result (AggregationFunction.extractFinalResult).  Values in one int order (larger = better for DESC):
+#   INT / LONG keys and COUNT: the integer; STRING keys: byte order (Java compareTo for ASCII);
+#   FLOAT / DOUBLE keys and SUM / AVG / MIN / MAX results: Double.compare (-0.0 < 0.0, NaN above +inf);
+#   MIN / MAX of a group without input: the +inf / -inf the hand-back emits (MinAggregationFunction / MaxAggregationFunction
+#   defaults); AVG of a group without input: AvgAggregationFunction.DEFAULT_FINAL_RESULT = Double.NEGATIVE_INFINITY.
+# Where the device's value is not exact (a float SUM / AVG), the order value is the interval every possible device value
+# lies in: check_sum's bound, plus one rounding for AVG's division.
+
+def order_double(x: float) -> int:
+    """Double.compare order as a signed int"""
+    if math.isnan(x):
+        return 0x7ff8000000000000
+    b = int(np.float64(x).view(np.int64))
+    return b if b >= 0 else b ^ 0x7fffffffffffffff
+
+
+def order_interval(q, key: tuple, row: list):
+    """(lo, hi) of the group's first ORDER BY value (a point where the device's value is exact)"""
+    kind, idx, _ = q.order_by[0]
+    if kind == 0:
+        v = key[idx]
+        v = order_double(v) if isinstance(v, float) else v
+        return v, v
+    agg, r = q.aggregations[idx], row[idx]
+    if agg.op == AggOp.COUNT:
+        return r, r
+    if agg.op in (AggOp.MIN, AggOp.MAX):
+        # a zero result is either zero: the strict compare keeps a group's first zero, and doc order is the device's to choose
+        return (order_double(-0.0), order_double(0.0)) if r == 0 else (order_double(r), order_double(r))
+    avg = agg.op == AggOp.AVG
+    ex = r.exact
+    if avg and r.n == 0:
+        v = order_double(-math.inf)
+        return v, v
+    if isinstance(ex, float) and not math.isfinite(ex):
+        v = order_double(ex)                       # (an infinite or NaN sum over n inputs: the average too)
+        return v, v
+    if r.integral and r.n * r.max_abs < 2.0 ** 53:  # every partial sum exact: the device's sum is exact, AVG one division
+        v = order_double(float(ex) / r.n if avg else float(ex))
+        return v, v
+    b = sum_bound(r)
+    lo, hi = float(ex) - b, float(ex) + b
+    if avg:
+        lo, hi = lo / r.n, hi / r.n
+    return order_double(lo - abs(lo) * 4 * U - 5e-324), order_double(hi + abs(hi) * 4 * U + 5e-324)
+
+
+def trim_bounds(lo, hi, size: int):
+    """(must, never) masks over groups with order intervals [lo, hi] (larger = better), keeping the `size` best with ties:
+    a group fewer than `size` others could beat must be kept; a group at least `size` others certainly beat is never kept.
+    With points both reduce to {g : v(g) >= v(size-th best)}."""
+    lo, hi = np.asarray(lo), np.asarray(hi)
+    n = len(lo)
+    could = n - np.searchsorted(np.sort(hi), lo, side="right") - (hi > lo)        # others h with hi_h > lo_g
+    certain = n - np.searchsorted(np.sort(lo), hi, side="right")                  # others h with lo_h > hi_g
+    return could < size, certain >= size
+
+
+def assert_trim_matches_reference(got_rows: Dict[tuple, list], ref: Dict[tuple, list], q, combined: bool, what="", complete=True):
+    """The returned groups are reference groups with matching values, and the trim kept the right ones: all of them when
+    no trim applies (at most the threshold or the trim size of groups: q.trim(combined)), else by trim_bounds.
+    complete=False: `ref` is a superset of the groups the trim ranked (a hash table that reached numGroupsLimit): the
+    returned groups are only checked for membership and values."""
+    extra = [k for k in got_rows if k not in ref]
+    assert not extra, f"{what}: groups not in the reference: {extra[:3]}"
+    assert_matches_reference(got_rows, {k: ref[k] for k in got_rows}, q, what)
+    size, thr = q.trim(combined)
+    if not complete:
+        return
+    if not size or len(ref) <= thr or len(ref) <= size:
+        assert len(got_rows) == len(ref), f"{what}: no trim applies to {len(ref)} groups, {len(got_rows)} returned"
+        return
+    keys = list(ref)
+    iv = [order_interval(q, k, ref[k]) for k in keys]
+    if isinstance(iv[0][0], bytes):                # STRING keys: their rank
+        rank = {v: i for i, v in enumerate(sorted({a for a, _ in iv}))}
+        iv = [(rank[a], rank[b]) for a, b in iv]
+    lo = np.array([a for a, _ in iv], dtype=np.int64)
+    hi = np.array([b for _, b in iv], dtype=np.int64)
+    if not q.order_by[0][2]:                       # ASC: smaller is better
+        lo, hi = ~hi, ~lo
+    must, never = trim_bounds(lo, hi, size)
+    kept = np.array([k in got_rows for k in keys])
+    missing = [keys[i] for i in np.flatnonzero(must & ~kept)]
+    wrong = [keys[i] for i in np.flatnonzero(never & kept)]
+    assert not missing and not wrong, f"{what}: trim to {size} of {len(ref)} groups kept {kept.sum()}: " \
+        f"missing {missing[:3]} (order {[order_interval(q, k, ref[k]) for k in missing[:3]]}), " \
+        f"kept beaten {wrong[:3]} (order {[order_interval(q, k, ref[k]) for k in wrong[:3]]})"
 
 
 def concat(tables, columns=None) -> Dict[str, Col]:

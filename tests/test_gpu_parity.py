@@ -480,8 +480,8 @@ def _expected_trim(rows, q, combined):
     def key(item):
         k, row = item
         v = k[idx] if kind == 0 else row[idx]
-        if isinstance(v, tuple):          # AVG: (sum, count)
-            v = v[0] / v[1] if v[1] else 0.0
+        if isinstance(v, tuple):          # AVG: (sum, count); no input: AvgAggregationFunction's DEFAULT_FINAL_RESULT
+            v = v[0] / v[1] if v[1] else float("-inf")
         return v
     vals = sorted((key(it) for it in rows.items()), reverse=desc)
     cut = vals[size - 1]
