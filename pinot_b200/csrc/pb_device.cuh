@@ -42,6 +42,16 @@ enum { T_KEYLESS = 0, T_DENSE = 1, T_HASH = 2 };
 
 #define PB_HASH_EMPTY 0xFFFFFFFFFFFFFFFFull
 
+// slots of a group table: a hash table has one more than its capacity, the reserved slot of the all-ones key
+__host__ __device__ __forceinline__ uint64_t pb_slots(int mode, uint64_t capacity) { return capacity + (mode == T_HASH ? 1 : 0); }
+
+// where group-by column j lives in a slot: dense slots are a mixed radix of the key fields (field = (slot / div) % card),
+// hash keys hold the fields side by side (bits [shift, shift + width) of the one or two key words)
+struct DevKeyField {
+  int32_t shift, width;
+  uint64_t div, card;
+};
+
 struct DevLeaf {
   int32_t kind;
   int32_t slot;            // scan slot (tile-staged column) for scan leaves
@@ -168,6 +178,11 @@ struct DevTable {
   uint32_t* first_doc;
   uint32_t num_groups_limit;
   uint32_t limit_active;             // 0: the table can never reach numGroupsLimit (limit >= docs), inserts need no ticket
+  // what the hand-back keeps (pb_slot_handed_back): groups whose first doc is <= *first_thr (when first_doc is tracked),
+  // and under an ORDER BY ... LIMIT trim those whose order key okey[slot] is >= *othr
+  uint32_t* first_thr;
+  unsigned long long* okey;
+  const unsigned long long* othr;
 };
 
 struct DevRowSeg;
@@ -554,7 +569,6 @@ __device__ __forceinline__ bool pb_group_ticket(const DevTable& t) {
   if (t.any_limit) pb_red_add_u32(t.any_limit, 1u);
   return false;
 }
-__device__ __forceinline__ void pb_group_ticket_return(const DevTable&) {}
 // The all-ones key has a reserved slot (t.capacity) instead of a claim in the key array; under a reachable limit its
 // first insert takes a ticket like any other new key.  (Racing first inserts may each take one: a lost ticket, as above.)
 __device__ __forceinline__ uint64_t pb_sentinel_slot(const DevTable& t, bool insert) {
@@ -578,8 +592,7 @@ __device__ __forceinline__ uint64_t pb_hash_slot(const DevTable& t, uint64_t key
       if (!insert || !pb_group_ticket(t)) return ~0ull;
       unsigned long long old = pb_atom_cas_u64(&t.hkeys[s], PB_HASH_EMPTY, (unsigned long long)key);
       if (old == PB_HASH_EMPTY) return s;
-      pb_group_ticket_return(t);                         // somebody else claimed the slot first
-      if (old == key) return s;
+      if (old == key) return s;                          // somebody else claimed the slot first
     }
     s = (s + 1) & mask;
   }
@@ -607,7 +620,6 @@ __device__ __forceinline__ uint64_t pb_hash_slot2(const DevTable& t, uint64_t lo
       unsigned long long olo, ohi;
       pb_atom_cas_u128(&t.hkeys[2 * s], PB_HASH_EMPTY, PB_HASH_EMPTY, lo, hi, olo, ohi);
       if (olo == PB_HASH_EMPTY && ohi == PB_HASH_EMPTY) return s;
-      pb_group_ticket_return(t);
       if (olo == lo && ohi == hi) return s;
     }
     s = (s + 1) & mask;
@@ -1929,19 +1941,43 @@ static __global__ void pb_merge_blocks_kernel(unsigned long long* __restrict__ d
 }
 
 // ------------------------------------------------------------------------------------------------
+// slots of a group table: what a slot holds, and which slots the hand-back returns
+// ------------------------------------------------------------------------------------------------
+// key words of hash slot i; the reserved slot at `capacity` holds the all-ones key, which has no entry in hkeys
+__device__ __forceinline__ void pb_slot_key(const DevTable& t, uint64_t i, unsigned long long& klo, unsigned long long& khi) {
+  if (t.key_words == 2) { klo = i == t.capacity ? PB_HASH_EMPTY : t.hkeys[2 * i]; khi = i == t.capacity ? PB_HASH_EMPTY : t.hkeys[2 * i + 1]; }
+  else { klo = i == t.capacity ? PB_HASH_EMPTY : t.hkeys[i]; khi = 0; }
+}
+// group-by field f of slot i (klo / khi: the slot's hash key, see pb_slot_key; a dense slot needs none)
+__device__ __forceinline__ uint64_t pb_slot_field(int mode, uint64_t i, unsigned long long klo, unsigned long long khi, const DevKeyField& f) {
+  if (mode == T_DENSE) return (i / f.div) % f.card;
+  uint64_t field;
+  if (f.shift < 64) { field = klo >> f.shift; if (f.shift && f.shift + f.width > 64) field |= khi << (64 - f.shift); }
+  else field = khi >> (f.shift - 64);
+  if (f.width < 64) field &= ((1ull << f.width) - 1ull);
+  return field;
+}
+// The hand-back rule.  A slot is admitted when it holds a group and the numGroupsLimit cut in doc order keeps it; the ORDER
+// BY ... LIMIT trim ranks the admitted groups only, and a slot is handed back when it is admitted and the trim keeps it.  A
+// keyless table always hands back its one slot, matches or not.  The group count that sizes the host arrays of a large
+// table and the finalize that fills them must agree on this, or rows past the count are lost.  (The thresholds are written
+// by earlier kernels, never by one that reads them: the read-only loads let a loop keep them in registers.)
+__device__ __forceinline__ bool pb_slot_admitted(const DevTable& t, uint64_t i) {
+  if (t.mode == T_KEYLESS) return true;
+  return t.rowcnt[i] != 0 && (!t.first_doc || t.first_doc[i] <= __ldg(t.first_thr));
+}
+__device__ __forceinline__ bool pb_slot_handed_back(const DevTable& t, uint64_t i) {
+  return pb_slot_admitted(t, i) && (!t.okey || t.okey[i] >= __ldg(t.othr));
+}
+
+// ------------------------------------------------------------------------------------------------
 // hash tables across ranks (SURVEY.md §8e: "partition tuples by hash(key) % nGPU, one all-to-all, local merge kernel"; the
 // reference merges by key in IndexedTable.upsert, CTR/data/table/IndexedTable.java:99-125).  A tuple is
 // [key words | row count | one u64 per aggregation (f64 sum bits / encoded min-max / filtered row count)].
 // ------------------------------------------------------------------------------------------------
 struct DevHashXfer {
-  int32_t n_ranks, key_words, n_aggs, tuple_words;
-  uint64_t S;                                   // slots to scan (capacity + the sentinel slot)
-  uint64_t capacity;
-  const unsigned long long* hkeys;
-  const unsigned long long* rowcnt;
-  const double* sum[PB_MAX_AGGS];
-  const long long* mm[PB_MAX_AGGS];
-  const unsigned long long* fcnt[PB_MAX_AGGS];
+  DevTable t;                                   // the local table
+  int32_t n_ranks, n_aggs, tuple_words, pad;
   unsigned long long* counts;                   // [n_ranks] tuples per destination
   unsigned long long* cursors;                  // [n_ranks] running positions while packing
   const unsigned long long* offsets;            // [n_ranks] first tuple of each destination in `out`
@@ -1952,31 +1988,28 @@ __device__ __forceinline__ uint32_t pb_owner_rank(unsigned long long klo, unsign
   unsigned long long h = pb_hash64((key_words == 2 ? (klo ^ pb_hash64(khi)) : klo) ^ 0x9e3779b97f4a7c15ull);
   return (uint32_t)((h >> 32) % (unsigned)n_ranks);
 }
-__device__ __forceinline__ void pb_slot_key(const DevHashXfer& X, uint64_t i, unsigned long long& klo, unsigned long long& khi) {
-  if (X.key_words == 2) { klo = i == X.capacity ? PB_HASH_EMPTY : X.hkeys[2 * i]; khi = i == X.capacity ? PB_HASH_EMPTY : X.hkeys[2 * i + 1]; }
-  else { klo = i == X.capacity ? PB_HASH_EMPTY : X.hkeys[i]; khi = 0; }
-}
 static __global__ void pb_hash_count_kernel(const DevHashXfer X) {
   __shared__ unsigned int s_cnt[64];
   for (int k = threadIdx.x; k < X.n_ranks; k += blockDim.x) s_cnt[k] = 0;
   __syncthreads();
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < X.S; i += (uint64_t)gridDim.x * blockDim.x) {
-    if (X.rowcnt[i] == 0) continue;
+  const uint64_t S = pb_slots(X.t.mode, X.t.capacity);
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < S; i += (uint64_t)gridDim.x * blockDim.x) {
+    if (X.t.rowcnt[i] == 0) continue;
     unsigned long long klo, khi;
-    pb_slot_key(X, i, klo, khi);
-    atomicAdd(&s_cnt[pb_owner_rank(klo, khi, X.key_words, X.n_ranks)], 1u);
+    pb_slot_key(X.t, i, klo, khi);
+    atomicAdd(&s_cnt[pb_owner_rank(klo, khi, X.t.key_words, X.n_ranks)], 1u);
   }
   __syncthreads();
   for (int k = threadIdx.x; k < X.n_ranks; k += blockDim.x) if (s_cnt[k]) atomicAdd(&X.counts[k], (unsigned long long)s_cnt[k]);
 }
 static __global__ void pb_hash_pack_kernel(const DevHashXfer X) {
   const int lane = threadIdx.x & 31;
-  const uint64_t S_round = (X.S + 31) & ~(uint64_t)31;
+  const uint64_t S = pb_slots(X.t.mode, X.t.capacity), S_round = (S + 31) & ~(uint64_t)31;
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < S_round; i += (uint64_t)gridDim.x * blockDim.x) {
-    const unsigned long long c = i < X.S ? X.rowcnt[i] : 0ull;
+    const unsigned long long c = i < S ? X.t.rowcnt[i] : 0ull;
     unsigned long long klo = 0, khi = 0;
     uint32_t dest = 0xffffffffu;
-    if (c) { pb_slot_key(X, i, klo, khi); dest = pb_owner_rank(klo, khi, X.key_words, X.n_ranks); }
+    if (c) { pb_slot_key(X.t, i, klo, khi); dest = pb_owner_rank(klo, khi, X.t.key_words, X.n_ranks); }
     // lanes bound for the same destination share one atomic
     const unsigned peers = __match_any_sync(0xffffffffu, dest);
     if (!c) continue;
@@ -1987,10 +2020,10 @@ static __global__ void pb_hash_pack_kernel(const DevHashXfer X) {
     unsigned long long* o = X.out + (X.offsets[dest] + base + __popc(peers & ((1u << lane) - 1u))) * (uint64_t)X.tuple_words;
     int w = 0;
     o[w++] = klo;
-    if (X.key_words == 2) o[w++] = khi;
+    if (X.t.key_words == 2) o[w++] = khi;
     o[w++] = c;
     for (int a = 0; a < X.n_aggs; a++)
-      o[w++] = X.sum[a] ? (unsigned long long)__double_as_longlong(X.sum[a][i]) : X.mm[a] ? (unsigned long long)X.mm[a][i] : X.fcnt[a] ? X.fcnt[a][i] : 0ull;
+      o[w++] = X.t.sum[a] ? (unsigned long long)__double_as_longlong(X.t.sum[a][i]) : X.t.mm[a] ? (unsigned long long)X.t.mm[a][i] : X.t.fcnt[a] ? X.t.fcnt[a][i] : 0ull;
   }
 }
 // received tuples -> this rank's (re-initialised) table
@@ -2082,78 +2115,64 @@ static __global__ void pb_invert_slots_kernel(const unsigned long long* __restri
 struct DevOrderKey {
   int32_t kind;              // 0 = group-by column, 1 = aggregation
   int32_t descending;
-  int32_t mode, key_words;   // table mode / hash key words
-  int32_t op;                // aggregation: PB_AGG_*
+  int32_t op, agg;           // aggregation: PB_AGG_* and its index in the table
   int32_t field_is_signed;   // group column: raw INT / LONG value (signed order)
   int32_t field_is_double;   // group column: raw FLOAT / DOUBLE value (bits of the double)
-  int32_t shift, width;      // hash: field position
-  uint64_t div, card;        // dense: field = (slot / div) % card
-  uint64_t S, capacity;
-  const unsigned long long* rowcnt;
-  const unsigned long long* hkeys;
-  const double* sum;
-  const long long* mm;
-  const unsigned long long* fcnt;
-  unsigned long long* okey;
+  DevKeyField field;         // group column: where it lives in a slot
 };
 // a double in Double.compare order (the order TableResizer sorts final results in): -0.0 < 0.0, and every NaN is one value
 // above +inf
 __device__ __forceinline__ long long pb_order_f64(double v) { return isnan(v) ? 0x7ff8000000000000LL : pb_enc_f64(v); }
-static __global__ void pb_order_key_kernel(const DevOrderKey K) {
+static __global__ void pb_order_key_kernel(const DevTable t, const DevOrderKey K) {
   const double inf = __longlong_as_double(0x7ff0000000000000LL);
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < K.S; i += (uint64_t)gridDim.x * blockDim.x) {
-    const unsigned long long c = K.rowcnt[i];
+  const double* sum = t.sum[K.agg];
+  const long long* mm = t.mm[K.agg];
+  const unsigned long long* fcnt = t.fcnt[K.agg];
+  const uint64_t S = pb_slots(t.mode, t.capacity);
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < S; i += (uint64_t)gridDim.x * blockDim.x) {
+    const unsigned long long c = t.rowcnt[i];
     unsigned long long u = 0;
     if (c) {
       if (K.kind == 1) {
         long long e;
-        if (K.op == 0) e = (long long)(K.fcnt ? K.fcnt[i] : c);                                        // COUNT
-        else if (K.op == 1) e = pb_order_f64(K.sum[i]);                                                 // SUM
+        if (K.op == 0) e = (long long)(fcnt ? fcnt[i] : c);                                            // COUNT
+        else if (K.op == 1) e = pb_order_f64(sum[i]);                                                   // SUM
         else if (K.op == 4) {                                                                           // AVG
           // no input (a FILTER clause left the group nothing): AvgAggregationFunction.extractFinalResult gives
           // DEFAULT_FINAL_RESULT = Double.NEGATIVE_INFINITY, below every real average
-          const unsigned long long n = K.fcnt ? K.fcnt[i] : c;
-          e = pb_order_f64(n ? K.sum[i] / (double)n : -inf);
+          const unsigned long long n = fcnt ? fcnt[i] : c;
+          e = pb_order_f64(n ? sum[i] / (double)n : -inf);
         }
-        else if (K.mm[i] == 0x7fffffffffffffffLL) e = pb_enc_f64(K.op == 2 ? inf : -inf);              // MIN / MAX without input: the +-inf the hand-back emits
-        else e = K.op == 2 ? K.mm[i] : ~K.mm[i];                                                        // MIN / MAX (encoded; MAX is stored complemented)
+        else if (mm[i] == 0x7fffffffffffffffLL) e = pb_enc_f64(K.op == 2 ? inf : -inf);                // MIN / MAX without input: the +-inf the hand-back emits
+        else e = K.op == 2 ? mm[i] : ~mm[i];                                                            // MIN / MAX (encoded; MAX is stored complemented)
         u = (unsigned long long)e ^ 0x8000000000000000ull;
       } else {
-        uint64_t field;
-        if (K.mode == T_DENSE) field = (i / K.div) % K.card;
-        else {
-          unsigned long long klo, khi = 0;
-          if (K.key_words == 2) { klo = i == K.capacity ? PB_HASH_EMPTY : K.hkeys[2 * i]; khi = i == K.capacity ? PB_HASH_EMPTY : K.hkeys[2 * i + 1]; }
-          else klo = i == K.capacity ? PB_HASH_EMPTY : K.hkeys[i];
-          if (K.shift < 64) { field = klo >> K.shift; if (K.shift && K.shift + K.width > 64) field |= khi << (64 - K.shift); }
-          else field = khi >> (K.shift - 64);
-          if (K.width < 64) field &= ((1ull << K.width) - 1ull);
-        }
+        unsigned long long klo = 0, khi = 0;
+        if (t.mode == T_HASH) pb_slot_key(t, i, klo, khi);
+        const uint64_t field = pb_slot_field(t.mode, i, klo, khi, K.field);
         if (K.field_is_double) u = (unsigned long long)pb_order_f64(__longlong_as_double((long long)field)) ^ 0x8000000000000000ull;
-        else if (K.field_is_signed) u = (K.width == 32 ? (unsigned long long)(long long)(int32_t)(uint32_t)field : field) ^ 0x8000000000000000ull;
+        else if (K.field_is_signed) u = (K.field.width == 32 ? (unsigned long long)(long long)(int32_t)(uint32_t)field : field) ^ 0x8000000000000000ull;
         else u = field;                                                                                  // dictId: sorted dictionary order
       }
       if (!K.descending) u = ~u;
     }
-    K.okey[i] = u;
+    t.okey[i] = u;
   }
 }
 // radix select, one 8-bit digit per pass: state = {prefix, k remaining, done, threshold, candidates}.  The candidates are the
-// groups the numGroupsLimit cut keeps (first_doc[slot] <= *first_thr, when the table tracks first docs): Pinot limits the
-// keys in the key generator and trims what is left.
+// admitted groups (pb_slot_admitted): Pinot limits the keys in the key generator and trims what is left.
 struct DevSelectState { unsigned long long prefix, k, done, thr, total; unsigned long long hist[256]; };
-static __global__ void pb_rselect_hist_kernel(const unsigned long long* __restrict__ okey, const unsigned long long* __restrict__ rowcnt, uint64_t S, int pass,
-                                              const uint32_t* __restrict__ first_doc, const uint32_t* __restrict__ first_thr, DevSelectState* st) {
+static __global__ void pb_rselect_hist_kernel(const DevTable t, int pass, DevSelectState* st) {
   __shared__ unsigned int h[256];
   for (int b = threadIdx.x; b < 256; b += blockDim.x) h[b] = 0;
   __syncthreads();
   if (!st->done) {
     const unsigned long long prefix = st->prefix;
     const unsigned long long hi_mask = pass == 7 ? 0ull : (~0ull << (8 * (pass + 1)));
-    const uint32_t fthr = first_doc ? *first_thr : 0u;
+    const uint64_t S = pb_slots(t.mode, t.capacity);
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < S; i += (uint64_t)gridDim.x * blockDim.x) {
-      if (!rowcnt[i] || (first_doc && first_doc[i] > fthr)) continue;
-      const unsigned long long v = okey[i];
+      if (!pb_slot_admitted(t, i)) continue;
+      const unsigned long long v = t.okey[i];
       if ((v & hi_mask) == (prefix & hi_mask)) atomicAdd(&h[(v >> (8 * pass)) & 255u], 1u);
     }
   }
@@ -2184,15 +2203,12 @@ static __global__ void pb_rselect_pick_kernel(DevSelectState* st, int pass, unsi
   for (int b = 0; b < 256; b++) st->hist[b] = 0;
 }
 
-// count non-empty slots (that survive the numGroupsLimit cut and the ORDER BY trim, if any)
-static __global__ void pb_count_groups_kernel(const unsigned long long* __restrict__ rowcnt, uint64_t n, unsigned long long* out,
-                                              const uint32_t* __restrict__ first_doc, const uint32_t* __restrict__ first_thr,
-                                              const unsigned long long* __restrict__ okey, const unsigned long long* __restrict__ othr) {
+// count the slots the hand-back returns
+static __global__ void pb_count_groups_kernel(const DevTable t, unsigned long long* out) {
   unsigned long long c = 0;
-  const unsigned long long thr = othr ? *othr : 0ull;
-  const uint32_t fthr = first_doc ? *first_thr : 0u;
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
-    c += rowcnt[i] != 0 && (!first_doc || first_doc[i] <= fthr) && (!okey || okey[i] >= thr);
+  const uint64_t S = pb_slots(t.mode, t.capacity);
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < S; i += (uint64_t)gridDim.x * blockDim.x)
+    c += pb_slot_handed_back(t, i);
   for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }
@@ -2205,33 +2221,21 @@ struct DevFinKey {
   int32_t eb;                 // bytes per decoded value
   int32_t is_dict;
   int32_t type;               // PB_INT .. PB_STRING
-  int32_t shift, width;       // T_HASH: field position in the composite key
   int32_t pad;
-  uint64_t div, card;         // T_DENSE: field = (slot / div) % card
+  DevKeyField field;
   int32_t* out_ids;
   uint8_t* out_vals;
 };
 struct DevFinAgg {
   int32_t op, pad;
-  const double* sum;
-  const long long* mm;
-  const unsigned long long* fcnt;   // COUNT / AVG with a FILTER clause: row count of the function (else the group's)
-  const unsigned long long* dcnt;   // DISTINCTCOUNT on a raw column: distinct values per slot
   double* out;
-  long long* out_cnt;               // where fcnt goes (the aggregation's long array)
+  long long* out_cnt;               // where the row count goes (the aggregation's long array)
 };
 struct DevFinalize {
-  int32_t mode, n_gb, n_aggs, always_emit;
-  uint64_t S;                 // slots to scan
-  int32_t key_words, count_all;   // count_all (PB_Q_NULL_HANDLING): every aggregation's long array carries its row count
-  uint64_t capacity;          // T_HASH: index of the reserved sentinel slot
+  DevTable t;
+  int32_t n_gb, n_aggs;
+  int32_t count_all, pad;     // count_all (PB_Q_NULL_HANDLING): every aggregation's long array carries its row count
   uint64_t cap_out;
-  const unsigned long long* rowcnt;
-  const unsigned long long* hkeys;
-  const uint32_t* first_doc;      // numGroupsLimit in doc order: emit only groups whose first doc is <= *first_thr
-  const uint32_t* first_thr;
-  const unsigned long long* okey; // ORDER BY ... LIMIT trim: emit only groups whose order key is >= *othr
-  const unsigned long long* othr;
   unsigned long long* cursor;
   unsigned long long* out_slots;
   unsigned long long* out_rows;
@@ -2240,14 +2244,13 @@ struct DevFinalize {
 };
 
 static __global__ void pb_finalize_kernel(const DevFinalize F) {
+  const DevTable& t = F.t;
   const int lane = threadIdx.x & 31;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-  const uint64_t S_round = (F.S + 31) & ~(uint64_t)31;
+  const uint64_t S = pb_slots(t.mode, t.capacity), S_round = (S + 31) & ~(uint64_t)31;
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < S_round; i += stride) {
-    const unsigned long long c = i < F.S ? F.rowcnt[i] : 0ull;
-    bool emit = i < F.S && (c != 0 || F.always_emit);
-    if (emit && F.first_doc && F.first_doc[i] > *F.first_thr) emit = false;
-    if (emit && F.okey && F.okey[i] < *F.othr) emit = false;
+    const unsigned long long c = i < S ? t.rowcnt[i] : 0ull;
+    const bool emit = i < S && pb_slot_handed_back(t, i);
     const uint32_t b = __ballot_sync(0xffffffffu, emit);
     if (!b) continue;
     unsigned long long base = 0;
@@ -2260,32 +2263,24 @@ static __global__ void pb_finalize_kernel(const DevFinalize F) {
     F.out_rows[k] = c;
     for (int a = 0; a < F.n_aggs; a++) {
       const DevFinAgg& fa = F.aggs[a];
-      if (fa.sum) fa.out[k] = fa.sum[i];
-      else if (fa.mm) {
+      const unsigned long long* fcnt = t.fcnt[a];
+      if (t.sum[a]) fa.out[k] = t.sum[a][i];
+      else if (t.mm[a]) {
         // empty group (keyless query without matches): MIN = +inf, MAX = -inf (MinAggregationFunction.java:37 defaults)
         // (same for a group none of whose docs passes the function's FILTER clause: the cell still holds the init pattern)
-        if (c == 0 || fa.mm[i] == 0x7fffffffffffffffLL) fa.out[k] = fa.op == 2 ? __longlong_as_double(0x7ff0000000000000LL) : __longlong_as_double((long long)0xfff0000000000000ULL);
-        else fa.out[k] = pb_dec_f64(fa.op == 2 ? fa.mm[i] : ~fa.mm[i]);
+        if (c == 0 || t.mm[a][i] == 0x7fffffffffffffffLL) fa.out[k] = fa.op == 2 ? __longlong_as_double(0x7ff0000000000000LL) : __longlong_as_double((long long)0xfff0000000000000ULL);
+        else fa.out[k] = pb_dec_f64(fa.op == 2 ? t.mm[a][i] : ~t.mm[a][i]);
       }
-      else if (fa.op == 0) fa.out[k] = fa.fcnt ? (double)fa.fcnt[i] : (double)c;
+      else if (fa.op == 0) fa.out[k] = fcnt ? (double)fcnt[i] : (double)c;
       // the aggregation's long array: COUNT value / AVG denominator (the function's own row count under a FILTER clause), 0 otherwise
-      if (fa.op == 5 && fa.dcnt) fa.out_cnt[k] = (long long)fa.dcnt[i];
-      if (fa.op != 5 && fa.out_cnt) fa.out_cnt[k] = (fa.op == 0 || fa.op == 4 || F.count_all) ? (fa.fcnt ? (long long)fa.fcnt[i] : (long long)c) : 0ll;
+      if (fa.op == 5 && t.dcnt[a]) fa.out_cnt[k] = (long long)t.dcnt[a][i];
+      if (fa.op != 5 && fa.out_cnt) fa.out_cnt[k] = (fa.op == 0 || fa.op == 4 || F.count_all) ? (fcnt ? (long long)fcnt[i] : (long long)c) : 0ll;
     }
     unsigned long long key = 0, key_hi = 0;
-    if (F.mode == T_HASH) {
-      if (F.key_words == 2) { key = (i == F.capacity) ? PB_HASH_EMPTY : F.hkeys[2 * i]; key_hi = (i == F.capacity) ? PB_HASH_EMPTY : F.hkeys[2 * i + 1]; }
-      else key = (i == F.capacity) ? PB_HASH_EMPTY : F.hkeys[i];
-    }
+    if (t.mode == T_HASH) pb_slot_key(t, i, key, key_hi);
     for (int j = 0; j < F.n_gb; j++) {
       const DevFinKey& fk = F.keys[j];
-      uint64_t field;
-      if (F.mode == T_DENSE) field = (i / fk.div) % fk.card;
-      else {
-        if (fk.shift < 64) { field = key >> fk.shift; if (fk.shift && fk.shift + fk.width > 64) field |= key_hi << (64 - fk.shift); }
-        else field = key_hi >> (fk.shift - 64);
-        if (fk.width < 64) field &= ((1ull << fk.width) - 1ull);
-      }
+      const uint64_t field = pb_slot_field(t.mode, i, key, key_hi, fk.field);
       uint8_t* o = fk.out_vals + k * (uint64_t)fk.eb;
       if (fk.is_dict) {
         fk.out_ids[k] = (int32_t)field;
@@ -2303,10 +2298,6 @@ static __global__ void pb_finalize_kernel(const DevFinalize F) {
   }
 }
 
-// gather kernels used by the two-pass path of very large tables
-static __global__ void pb_gather_u64_kernel(const unsigned long long* __restrict__ src, const unsigned long long* __restrict__ slots, uint64_t n, unsigned long long* __restrict__ dst) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) dst[i] = src[slots[i]];
-}
 // DISTINCTCOUNT: one warp per compacted group: popcount of its bitset
 static __global__ void pb_distinct_count_kernel(const uint32_t* __restrict__ bits, uint64_t words, const unsigned long long* __restrict__ slots,
                                          uint64_t n, unsigned long long* __restrict__ out) {

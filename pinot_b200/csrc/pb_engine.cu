@@ -993,8 +993,7 @@ struct TableMeta {
   int mode = 0;
   uint64_t capacity = 0;
   std::vector<int> seg_idx;                 // segments accumulated into this table
-  std::vector<int64_t> cards;               // per group-by column (global or local)
-  std::vector<int> shifts, widths;          // hash key layout
+  std::vector<DevKeyField> fields;          // per group-by column: its place in a slot (card: global or local, ~0 for a raw column)
   DevTable dev;                             // device pointers (host copy of the struct)
   // finalize outputs
   int64_t num_groups = 0;
@@ -1073,10 +1072,10 @@ struct pb_result_s {
                     uint4* aux = nullptr; uint64_t an = 0; const uint4* head = nullptr; uint64_t head_n16 = 0; int grid = 1; } init;   // pb_init_tables_kernel
   int key_words = 1;
   int32_t plan_info[PB_PLAN_INFO_N] = {0};  // pb_result_plan_info, filled by plan_launches
-  // ORDER BY ... LIMIT trim (pb_query_desc.order_by): per table an order-key array and the radix-select state
+  // ORDER BY ... LIMIT trim (pb_query_desc.order_by): per table the radix-select state (the order keys: DevTable::okey)
   pb_order_by order0{0, 0, 0}; int trim_size = 0, trim_threshold = 0;
-  std::vector<unsigned long long*> d_okey; std::vector<DevSelectState*> d_sel;
-  bool track_first = false; uint32_t* d_first_thr = nullptr;   // numGroupsLimit in doc order (dense per-segment tables)
+  std::vector<DevSelectState*> d_sel;
+  bool track_first = false;                 // numGroupsLimit in doc order (dense per-segment tables)
   bool repair_pass = false;                 // hash tables with a reachable numGroupsLimit: conditional second aggregation pass
   bool comm_timed = false;                  // events [5],[6] bracket the cross-rank merge
   double comm_ms = 0;
@@ -1869,7 +1868,6 @@ static int stage_inputs(Plan& P) {
   return PB_OK;
 }
 
-static uint64_t slots_of(const Plan& P, const TableMeta& tm) { return tm.capacity + (P.r->table_mode == T_HASH ? 1 : 0); }
 static uint64_t table_docs(const Plan& P, const TableMeta& tm) {
   uint64_t docs = 0;
   for (int si : tm.seg_idx) docs += (uint64_t)P.g->segs[si]->num_docs;
@@ -1897,9 +1895,10 @@ static int plan_table_mode(Plan& P) {
     for (int t = 0; t < P.n_tables; t++) {
       TableMeta& tm = r->tables[t];
       int si0 = P.combine ? 0 : t;
-      tm.cards.resize(nG); tm.shifts.resize(nG); tm.widths.resize(nG);
+      tm.fields.resize(nG);
       unsigned __int128 prod = 1;
       int total_bits = 0;
+      uint64_t div = 1;
       for (int j = 0; j < nG; j++) {
         const Column& c = P.g->segs[si0]->cols[P.gcol[si0][j]];
         int64_t card; int width;
@@ -1911,7 +1910,9 @@ static int plan_table_mode(Plan& P) {
           width = (c.type == PB_INT || c.type == PB_FLOAT) ? 32 : 64;
           if (nG == 1) width = 64;
         }
-        tm.cards[j] = card; tm.widths[j] = width; tm.shifts[j] = total_bits; total_bits += width;
+        tm.fields[j] = {total_bits, width, div, (uint64_t)card};
+        total_bits += width;
+        if (card > 0) div *= (uint64_t)card;
         if (card > 0 && prod <= ((unsigned __int128)1 << 70)) prod *= (unsigned __int128)card;
       }
       bool dense_ok = !P.any_raw_key && prod <= PB_DENSE_MAX;
@@ -1977,7 +1978,7 @@ static int lay_out_tables(Plan& P) {
   size_t zo = tables_off, fo = 0, mo = 0;
   for (int t = 0; t < P.n_tables; t++) {
     TableMeta& tm = r->tables[t];
-    const uint64_t S = slots_of(P, tm);
+    const uint64_t S = pb_slots(tm.mode, tm.capacity);
     DevTable& dt = tm.dev;
     memset(&dt, 0, sizeof dt);
     dt.mode = r->table_mode; dt.capacity = tm.capacity;
@@ -2047,7 +2048,6 @@ static int alloc_tables(Plan& P) {
   CU(cudaMallocAsync((void**)&P.d_zero, P.zero_bytes + mm_bytes + P.aux_bytes + 16, st)); r->dev_allocs.push_back(P.d_zero);
   if (P.ff_bytes) { CU(cudaMallocAsync((void**)&P.d_ff, P.ff_bytes + 16, st)); r->dev_allocs.push_back(P.d_ff); }
   P.d_aux = P.d_zero + P.zero_bytes + mm_bytes;
-  r->d_first_thr = r->track_first ? reinterpret_cast<uint32_t*>(P.d_aux + thr_off) : nullptr;
   r->block = P.d_zero; r->block_bytes = (int64_t)(P.zero_bytes + 8 * P.mm_elems);
   r->block_mm_off = (int64_t)P.zero_bytes;
   r->d_counters = reinterpret_cast<unsigned long long*>(P.d_zero);
@@ -2055,15 +2055,17 @@ static int alloc_tables(Plan& P) {
   if ((rc = lay_out_tables(P))) return rc;
   CU(cudaGetLastError());
 
-  if (r->trim_size > 0) {
-    for (int t = 0; t < P.n_tables; t++) {
-      const uint64_t S = slots_of(P, r->tables[t]);
-      unsigned long long* ok = nullptr; DevSelectState* sel = nullptr;
-      CU(cudaMallocAsync((void**)&ok, 8 * S, st)); r->dev_allocs.push_back(ok);
-      CU(cudaMallocAsync((void**)&sel, sizeof(DevSelectState), st)); r->dev_allocs.push_back(sel);
-      CU(cudaMemsetAsync(sel, 0, sizeof(DevSelectState), st));
-      r->d_okey.push_back(ok); r->d_sel.push_back(sel);
-    }
+  // what the hand-back reads besides the table (pb_slot_handed_back), set before alloc_arena copies the tables
+  for (int t = 0; t < P.n_tables; t++) {
+    DevTable& dt = r->tables[t].dev;
+    if (dt.first_doc) dt.first_thr = reinterpret_cast<uint32_t*>(P.d_aux + thr_off) + t;
+    if (r->trim_size <= 0) continue;
+    DevSelectState* sel = nullptr;
+    CU(cudaMallocAsync((void**)&dt.okey, 8 * pb_slots(dt.mode, dt.capacity), st)); r->dev_allocs.push_back(dt.okey);
+    CU(cudaMallocAsync((void**)&sel, sizeof(DevSelectState), st)); r->dev_allocs.push_back(sel);
+    CU(cudaMemsetAsync(sel, 0, sizeof(DevSelectState), st));
+    dt.othr = &sel->thr;
+    r->d_sel.push_back(sel);
   }
   return PB_OK;
 }
@@ -2311,7 +2313,6 @@ static int bind_segment(Plan& P, int si) {
   // group-by / aggregation columns
   const TableMeta& tm = P.r->tables[ds.table];
   const RowGroup* rg = P.seg_rg[si];
-  uint64_t mult = 1;
   for (int j = 0; j < nG; j++) {
     const Column& c = s->cols[P.gcol[si][j]];
     DevKeyCol& kc = ds.keys[j];
@@ -2320,9 +2321,8 @@ static int bind_segment(Plan& P, int si) {
     kc.bits = c.bits; kc.raw_width = c.has_dict ? 0 : c.raw_width; kc.data_type = c.type;
     kc.stride_bits = src.stride_bits; kc.bit_off = src.bit_off;
     kc.remap = (P.combine && P.gdict[j] && !P.gdict[j]->identity[si]) ? P.gdict[j]->d_remap[si] : nullptr;
-    kc.shift = tm.shifts[j];
-    kc.mult = mult;
-    if (tm.cards[j] > 0) mult *= (uint64_t)tm.cards[j];
+    kc.shift = tm.fields[j].shift;
+    kc.mult = tm.fields[j].div;
     if (!c.has_dict && (c.type == PB_FLOAT) && nG > 1) return fail(PB_ERR_UNSUPPORTED, "raw FLOAT key in a multi-column group-by");
   }
   for (int a = 0; a < P.nA; a++) {
@@ -2494,7 +2494,7 @@ static int fill_counters_head(Plan& P) {
   mix((unsigned long long)r->block_bytes); mix((unsigned long long)r->block_sum_off); mix((unsigned long long)r->block_dc_off); mix((unsigned long long)r->block_mm_off);
   mix((unsigned long long)r->table_mode); mix((unsigned long long)P.nG); mix((unsigned long long)P.nA); mix((unsigned long long)P.nF);
   for (int a = 0; a < P.nA; a++) mix((unsigned long long)q->aggregations[a].op * 131 + P.dc_words[a]);
-  for (auto& tm : r->tables) { mix(tm.capacity); for (auto cd : tm.cards) mix((unsigned long long)cd); }
+  for (auto& tm : r->tables) { mix(tm.capacity); for (auto& f : tm.fields) mix(f.card); }
   r->fingerprint = fp >> 8;                               // head room: n_ranks x fp must not wrap
   for (int t = 0; t < P.n_tables; t++) h_head[(size_t)t * PB_COUNTERS_PER_TABLE + 9] = r->fingerprint;
   return PB_OK;
@@ -2982,7 +2982,7 @@ static int enqueue_trim(pb_result_s* r) {
   for (size_t t = 0; t < r->tables.size(); t++) {
     const DevTable& dt = r->tables[t].dev;
     if (!dt.first_doc) continue;
-    pb_select_first_kernel<<<1, 1024, 0, st>>>(dt.first_doc, r->tables[t].capacity, dt.num_groups_limit, r->d_first_thr + t);
+    pb_select_first_kernel<<<1, 1024, 0, st>>>(dt.first_doc, r->tables[t].capacity, dt.num_groups_limit, dt.first_thr);
     r->launches++;
   }
   CU(cudaGetLastError());
@@ -2991,26 +2991,21 @@ static int enqueue_trim(pb_result_s* r) {
   for (size_t t = 0; t < r->tables.size(); t++) {
     TableMeta& tm = r->tables[t];
     DevOrderKey K; memset(&K, 0, sizeof K);
-    K.kind = r->order0.kind; K.descending = r->order0.descending; K.mode = r->table_mode; K.key_words = tm.dev.key_words;
-    K.S = tm.capacity + (r->table_mode == T_HASH ? 1 : 0); K.capacity = tm.capacity;
-    K.rowcnt = tm.dev.rowcnt; K.hkeys = tm.dev.hkeys; K.okey = r->d_okey[t];
+    K.kind = r->order0.kind; K.descending = r->order0.descending;
     if (K.kind == 1) {
-      const int a = r->order0.index;
-      K.op = r->agg_op[a]; K.sum = tm.dev.sum[a]; K.mm = tm.dev.mm[a]; K.fcnt = tm.dev.fcnt[a];
+      K.agg = r->order0.index; K.op = r->agg_op[K.agg];
     } else {
       const int j = r->order0.index;
       const pb_segment_s* s0 = g->segs[tm.seg_idx[0]];
       const Column& c0 = s0->cols[find_col(s0, r->gb_names[j].c_str())];
       K.field_is_signed = !c0.has_dict && (c0.type == PB_INT || c0.type == PB_LONG);
       K.field_is_double = !c0.has_dict && (c0.type == PB_FLOAT || c0.type == PB_DOUBLE);
-      if (r->table_mode == T_DENSE) { uint64_t div = 1; for (int k = 0; k < j; k++) div *= (uint64_t)tm.cards[k]; K.div = div; K.card = (uint64_t)tm.cards[j]; }
-      else { K.shift = tm.shifts[j]; K.width = tm.widths[j]; }
+      K.field = tm.fields[j];
     }
-    const int grid = (int)std::min<uint64_t>((K.S + 255) / 256, (uint64_t)r->ctx->num_sms * 8);
-    pb_order_key_kernel<<<grid, 256, 0, st>>>(K);
-    const uint32_t* first_thr = tm.dev.first_doc ? r->d_first_thr + t : nullptr;
+    const int grid = (int)std::min<uint64_t>((pb_slots(tm.mode, tm.capacity) + 255) / 256, (uint64_t)r->ctx->num_sms * 8);
+    pb_order_key_kernel<<<grid, 256, 0, st>>>(tm.dev, K);
     for (int pass = 7; pass >= 0; pass--) {
-      pb_rselect_hist_kernel<<<grid, 256, 0, st>>>(K.okey, K.rowcnt, K.S, pass, tm.dev.first_doc, first_thr, r->d_sel[t]);
+      pb_rselect_hist_kernel<<<grid, 256, 0, st>>>(tm.dev, pass, r->d_sel[t]);
       pb_rselect_pick_kernel<<<1, 32, 0, st>>>(r->d_sel[t], pass, (unsigned long long)r->trim_size, (unsigned long long)r->trim_threshold,
                                                (unsigned long long)tm.dev.num_groups_limit, tm.dev.limit_reached);
     }
@@ -3037,13 +3032,11 @@ static int prepare_finalize(pb_result_s* r) {
   bool any_big = false;
   for (int t = 0; t < nT; t++) {
     TableMeta& tm = r->tables[t];
-    const uint64_t S = tm.capacity + (mode == T_HASH ? 1 : 0);
+    const uint64_t S = pb_slots(mode, tm.capacity);
     if (mode != T_KEYLESS && S > SMALL_TABLE) {
       any_big = true;
       int grid = (int)std::min<uint64_t>((S + 255) / 256, 2048);
-      pb_count_groups_kernel<<<grid, 256, 0, st>>>(tm.dev.rowcnt, S, r->d_counters + (size_t)t * PB_COUNTERS_PER_TABLE + 3,
-                                                   tm.dev.first_doc, tm.dev.first_doc ? r->d_first_thr + t : nullptr,
-                                                   r->trim_size > 0 ? r->d_okey[(size_t)t] : nullptr, r->trim_size > 0 ? &r->d_sel[(size_t)t]->thr : nullptr);
+      pb_count_groups_kernel<<<grid, 256, 0, st>>>(tm.dev, r->d_counters + (size_t)t * PB_COUNTERS_PER_TABLE + 3);
       r->launches++;
     }
   }
@@ -3056,8 +3049,8 @@ static int prepare_finalize(pb_result_s* r) {
   rp.fin_grid.assign((size_t)nT, 1);
   for (int t = 0; t < nT; t++) {
     TableMeta& tm = r->tables[t];
-    const uint64_t S = tm.capacity + (mode == T_HASH ? 1 : 0);
-    uint64_t cap = mode == T_KEYLESS ? 1 : S;
+    const uint64_t S = pb_slots(mode, tm.capacity);
+    uint64_t cap = S;
     if (mode != T_KEYLESS && S > SMALL_TABLE) {
       cap = std::max<uint64_t>(hc[(size_t)t * PB_COUNTERS_PER_TABLE + 3], 1);
       CU(cudaMemsetAsync(r->d_counters + (size_t)t * PB_COUNTERS_PER_TABLE + 3, 0, 8, st));
@@ -3069,11 +3062,7 @@ static int prepare_finalize(pb_result_s* r) {
     if (!tm.slots.p || !tm.rows.p) return fail(PB_ERR_OOM, "pinned host allocation failed");
     DevFinalize& F = rp.fin[(size_t)t];
     memset(&F, 0, sizeof F);
-    F.mode = mode; F.n_gb = nG; F.n_aggs = nA; F.always_emit = mode == T_KEYLESS ? 1 : 0; F.count_all = r->count_all ? 1 : 0;
-    F.S = mode == T_KEYLESS ? 1 : S; F.capacity = tm.capacity; F.cap_out = cap; F.key_words = tm.dev.key_words;
-    F.rowcnt = tm.dev.rowcnt; F.hkeys = tm.dev.hkeys;
-    if (tm.dev.first_doc) { F.first_doc = tm.dev.first_doc; F.first_thr = r->d_first_thr + t; }
-    if (r->trim_size > 0 && mode != T_KEYLESS) { F.okey = r->d_okey[(size_t)t]; F.othr = &r->d_sel[(size_t)t]->thr; }
+    F.t = tm.dev; F.n_gb = nG; F.n_aggs = nA; F.count_all = r->count_all ? 1 : 0; F.cap_out = cap;
     F.cursor = r->d_counters + (size_t)t * PB_COUNTERS_PER_TABLE + 3;
     // every byte of the hand-back crosses PCIe: the slot of a row is only written when a DISTINCTCOUNT will ask for it, and
     // the long arrays of SUM / MIN / MAX (all zeros) are made on the host when somebody reads them (pb_result_long)
@@ -3083,11 +3072,10 @@ static int prepare_finalize(pb_result_s* r) {
     for (int a = 0; a < nA; a++) {
       tm.dbl[a].alloc(8 * cap); tm.lng[a].alloc(8 * cap);
       if (!tm.dbl[a].p || !tm.lng[a].p) return fail(PB_ERR_OOM, "pinned host allocation failed");
-      F.aggs[a].op = r->agg_op[a]; F.aggs[a].sum = tm.dev.sum[a]; F.aggs[a].mm = tm.dev.mm[a]; F.aggs[a].out = (double*)tm.dbl[a].p;
+      F.aggs[a].op = r->agg_op[a]; F.aggs[a].out = (double*)tm.dbl[a].p;
       const bool lng_on_device = r->agg_op[a] == PB_AGG_COUNT || r->agg_op[a] == PB_AGG_AVG || r->agg_op[a] == PB_AGG_DISTINCTCOUNT || r->count_all;
-      F.aggs[a].fcnt = tm.dev.fcnt[a]; F.aggs[a].out_cnt = lng_on_device ? (long long*)tm.lng[a].p : nullptr; F.aggs[a].dcnt = tm.dev.dcnt[a];
+      F.aggs[a].out_cnt = lng_on_device ? (long long*)tm.lng[a].p : nullptr;
     }
-    uint64_t div = 1;
     for (int j = 0; j < nG; j++) {
       const pb_segment_s* s0 = g->segs[tm.seg_idx[0]];
       const Column& c0 = s0->cols[find_col(s0, r->gb_names[j].c_str())];
@@ -3098,14 +3086,13 @@ static int prepare_finalize(pb_result_s* r) {
         else { fk.dict_vals = c0.d_dict_native; fk.eb = c0.entry_bytes; }
         if (!fk.dict_vals) return fail(PB_ERR_STATE, "dictionary of %s is not staged", c0.name.c_str());
       } else fk.eb = (c0.type == PB_INT || c0.type == PB_FLOAT) ? 4 : 8;
-      if (mode == T_DENSE) { fk.div = div; fk.card = (uint64_t)tm.cards[j]; div *= (uint64_t)tm.cards[j]; }
-      else if (mode == T_HASH) { fk.shift = tm.shifts[j]; fk.width = tm.widths[j]; }
+      fk.field = tm.fields[j];
       tm.key_type[j] = c0.type; tm.key_eb[j] = fk.eb;
       tm.key_ids[j].alloc(4 * cap); tm.key_vals[j].alloc((size_t)fk.eb * cap);
       if (!tm.key_ids[j].p || !tm.key_vals[j].p) return fail(PB_ERR_OOM, "pinned host allocation failed");
       fk.out_ids = (int32_t*)tm.key_ids[j].p; fk.out_vals = (uint8_t*)tm.key_vals[j].p;
     }
-    rp.fin_grid[(size_t)t] = (int)std::min<uint64_t>((F.S + 255) / 256, 1184);
+    rp.fin_grid[(size_t)t] = (int)std::min<uint64_t>((S + 255) / 256, 1184);
   }
   rp.fin_prepared = true;
   return PB_OK;
@@ -3276,7 +3263,7 @@ static int materialize_distinct(pb_result_s* r, TableMeta& tm, int a) {
     tm.dc_vals[a].alloc(8 * (size_t)std::max<int64_t>(total, 1));
     if (!tm.dc_vals[a].p) return fail(PB_ERR_OOM, "pinned host allocation failed");
     if (total > 0) {
-      const uint64_t S = tm.capacity + (r->table_mode == T_HASH ? 1 : 0), cap = tm.dev.dset_mask[a] + 1;
+      const uint64_t S = pb_slots(tm.mode, tm.capacity), cap = tm.dev.dset_mask[a] + 1;
       uint32_t* d_map = nullptr; unsigned long long* d_cur = nullptr;
       CU(cudaMallocAsync((void**)&d_map, 4 * S, st));
       CU(cudaMallocAsync((void**)&d_cur, 8 * (size_t)ng, st));
@@ -3351,8 +3338,7 @@ static int comm_merge_hash(pb_result_s* r) {
   cudaStream_t st = r->stream;
   Context* ctx = r->ctx;
   const int kw = r->key_words, T = kw + 1 + nA;
-  const uint64_t S = tm.capacity + 1;
-  const int grid = (int)std::min<uint64_t>((S + 255) / 256, (uint64_t)ctx->num_sms * 8);
+  const int grid = (int)std::min<uint64_t>((pb_slots(tm.mode, tm.capacity) + 255) / 256, (uint64_t)ctx->num_sms * 8);
   CU(cudaEventRecord(r->sset.ev[5], st));
   // small control block: [counts n | cursors n | offsets n | all counts n*n | counter cells n*PB_COUNTERS_PER_TABLE]
   const size_t ctl_words = (size_t)3 * n + (size_t)n * n + (size_t)n * PB_COUNTERS_PER_TABLE + 8;
@@ -3361,9 +3347,7 @@ static int comm_merge_hash(pb_result_s* r) {
   CU(cudaMemsetAsync(d_ctl, 0, 8 * ctl_words, st));
   unsigned long long *d_counts = d_ctl, *d_cursors = d_ctl + n, *d_offsets = d_ctl + 2 * n, *d_all = d_ctl + 3 * n, *d_cells = d_ctl + 3 * n + (size_t)n * n;
   DevHashXfer X; memset(&X, 0, sizeof X);
-  X.n_ranks = n; X.key_words = kw; X.n_aggs = nA; X.tuple_words = T; X.S = S; X.capacity = tm.capacity;
-  X.hkeys = tm.dev.hkeys; X.rowcnt = tm.dev.rowcnt;
-  for (int a = 0; a < nA; a++) { X.sum[a] = tm.dev.sum[a]; X.mm[a] = tm.dev.mm[a]; X.fcnt[a] = tm.dev.fcnt[a]; }
+  X.t = tm.dev; X.n_ranks = n; X.n_aggs = nA; X.tuple_words = T;
   X.counts = d_counts; X.cursors = d_cursors; X.offsets = d_offsets;
   pb_hash_count_kernel<<<grid, 256, 0, st>>>(X);
   r->launches++;
