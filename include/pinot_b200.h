@@ -296,19 +296,15 @@ int32_t pb_result_plan_info(pb_result_handle r, int32_t* out, int32_t n);
 int pb_result_host_timing(pb_result_handle r, double* out8);
 void pb_result_free(pb_result_handle r);
 
-/* -------- multi-GPU (PB_Q_COMBINE | PB_Q_DEFER_FINALIZE): device-resident table arrays for an
- * NCCL all-reduce issued by the caller (torch.distributed), then finalize on the root.
- * which: 0 = row counts (int64, SUM); 1 = per-aggregation double sums (float64, SUM);
- *        2 = per-aggregation min/max in order-preserving int64 encoding (int64; reduce with MIN for both:
- *            MAX tables hold the bit-complement);
- *        5 / 6 / 7 = the same data as three contiguous spans, one collective each: 5 = counters + row counts
- *            (int64, SUM), 6 = all sums (float64, SUM; may be empty), 7 = all min/max tables (int64, MIN; may be empty);
- *        3 = per-aggregation distinct bitset words (int32; OR == MAX over 0/1 is NOT valid — all-gather + pb_or) -------- */
+/* -------- multi-GPU (PB_Q_COMBINE | PB_Q_DEFER_FINALIZE): a merge driven by a caller with its own collective library.
+ * which = 8 (the only buffer; `agg` is ignored): the whole reducible state of a keyless or dense table as one byte block
+ * (num_elements = bytes; a hash table is PB_ERR_UNSUPPORTED).  Wait for the result, check that the size is the same on every
+ * rank, all-gather the block across ranks (one collective) and hand the rank-major copies to pb_result_merge_gathered, which
+ * reduces them into this result on the result's stream with the right operator per region (u64 SUM | f64 SUM | bitset OR |
+ * i64 MIN) and records how many ranks went in; then pb_result_finalize, which fails with PB_ERR_STATE when the ranks' layouts
+ * differed.  An all-reduce of the block's regions is not offered: no reduction operator ORs the DISTINCTCOUNT bitsets, and
+ * the block's layout fingerprint must be checked against the number of ranks merged. -------- */
 int pb_result_device_buffer(pb_result_handle r, int32_t which, int32_t agg, void** device_ptr, int64_t* num_elements);
-/* which = 8: the whole reducible state of the table as one byte block (num_elements = bytes).  all-gather it across
- * ranks (one collective) and hand the rank-major copies to pb_result_merge_gathered, which reduces them into this result on
- * the result's stream with the right operator per region (u64 SUM | f64 SUM | bitset OR | i64 MIN) — this also merges
- * DISTINCTCOUNT bitsets, which no NCCL reduction operator can. */
 int pb_result_merge_gathered(pb_result_handle r, const void* gathered_device_ptr, int32_t n_ranks);
 int pb_result_finalize(pb_result_handle r);
 /* the CUDA stream (cudaStream_t) this result's work was issued on, and a host-side wait for it */

@@ -1035,10 +1035,6 @@ struct pb_result_s {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, ev2 = nullptr, ev3 = nullptr;
   StreamSet sset;
   double filter_ms = 0, agg_ms = 0;
-  // contiguous spans of table 0 for the cross-GPU reduce: [counters .. row counts] int64 SUM, sums float64 SUM, min/max int64 MIN
-  unsigned long long* span_i64 = nullptr; int64_t span_i64_n = 0;
-  double* span_f64 = nullptr; int64_t span_f64_n = 0;
-  long long* span_mm = nullptr; int64_t span_mm_n = 0;
   // the whole reducible state of table 0 as one block: [0, sum_off) counters + row counts (u64 SUM), [sum_off, dc_off) sums
   // (f64 SUM), [dc_off, mm_off) distinct bitsets (OR), [mm_off, bytes) min/max (i64 MIN)
   uint8_t* block = nullptr; int64_t block_bytes = 0, block_sum_off = 0, block_dc_off = 0, block_mm_off = 0;
@@ -1985,20 +1981,19 @@ static int lay_out_tables(Plan& P) {
     dt.rowcnt = static_cast<unsigned long long*>(zp(zo)); zo += 8 * S;
     for (int a = 0; a < nA; a++)     // (u64, summed across GPUs with the row counts)
       if (has_fcnt(q, a)) { dt.fcnt[a] = static_cast<unsigned long long*>(zp(zo)); zo += 8 * S; }
-    if (t == 0) { r->span_i64 = static_cast<unsigned long long*>(zp(0)); r->span_i64_n = (int64_t)(zo / 8); r->block_sum_off = (int64_t)zo; }
+    if (t == 0) r->block_sum_off = (int64_t)zo;
     // sums first (one contiguous float64 span for the cross-GPU reduce), then the distinct bitsets
     for (int a = 0; a < nA; a++) {
       int op = q->aggregations[a].op;
       if (op == PB_AGG_SUM || op == PB_AGG_AVG) { dt.sum[a] = static_cast<double*>(zp(zo)); zo += 8 * S; }
     }
-    if (t == 0) { r->span_f64 = static_cast<double*>(zp((size_t)r->block_sum_off)); r->span_f64_n = (int64_t)((zo - (size_t)r->block_sum_off) / 8); r->block_dc_off = (int64_t)zo; }
+    if (t == 0) r->block_dc_off = (int64_t)zo;
     for (int a = 0; a < nA; a++) {
       int op = q->aggregations[a].op;
       if (op == PB_AGG_DISTINCTCOUNT && !P.dc_raw[a]) { dt.dc_bits[a] = static_cast<uint32_t*>(zp(zo)); dt.dc_words[a] = P.dc_words[a]; zo += 4 * S * P.dc_words[a]; }
       if (op == PB_AGG_DISTINCTCOUNT && P.dc_raw[a]) { dt.dcnt[a] = static_cast<unsigned long long*>(zp(zo)); zo += 8 * S; }
       if (op == PB_AGG_MIN || op == PB_AGG_MAX) { dt.mm[a] = d_mm ? d_mm + mo : nullptr; mo += S; }
     }
-    if (t == 0) { r->span_mm = d_mm; r->span_mm_n = (int64_t)mo; }
     zo = (zo + 255) & ~(size_t)255;
     // every piece of the 0xFF region starts 16-byte aligned (CAS.128)
     if (r->table_mode == T_HASH) { dt.hkeys = static_cast<unsigned long long*>(fp(fo)); fo += (8 * S * (size_t)r->key_words + 15) & ~(size_t)15; dt.key_words = r->key_words; }
@@ -2982,6 +2977,9 @@ static int enqueue_trim(pb_result_s* r) {
   for (size_t t = 0; t < r->tables.size(); t++) {
     const DevTable& dt = r->tables[t].dev;
     if (!dt.first_doc) continue;
+    // a merged table also holds groups of other ranks, which have no first doc here: like the merged table of several
+    // segments it hands back every group and the flag
+    if (r->merged_ranks > 1) { CU(cudaMemsetAsync(dt.first_thr, 0xff, 4, st)); continue; }
     pb_select_first_kernel<<<1, 1024, 0, st>>>(dt.first_doc, r->tables[t].capacity, dt.num_groups_limit, dt.first_thr);
     r->launches++;
   }
@@ -3466,21 +3464,11 @@ extern "C" int pb_result_device_buffer(pb_result_handle r, int32_t which, int32_
   if (!r || !device_ptr || !num_elements) return fail(PB_ERR_INVALID, "null argument");
   if (!r->combine || r->tables.size() != 1) return fail(PB_ERR_STATE, "device buffers are exposed for PB_Q_COMBINE results only");
   if (r->table_mode == T_HASH) return fail(PB_ERR_UNSUPPORTED, "hash tables cannot be all-reduced in place");
-  TableMeta& tm = r->tables[0];
-  const int64_t S = (int64_t)tm.capacity;
-  switch (which) {
-    case 0: *device_ptr = tm.dev.rowcnt; *num_elements = S; return PB_OK;
-    case 1: if (agg < 0 || agg >= r->n_aggs || !tm.dev.sum[agg]) break; *device_ptr = tm.dev.sum[agg]; *num_elements = S; return PB_OK;
-    case 2: if (agg < 0 || agg >= r->n_aggs || !tm.dev.mm[agg]) break; *device_ptr = tm.dev.mm[agg]; *num_elements = S; return PB_OK;
-    case 3: if (agg < 0 || agg >= r->n_aggs || !tm.dev.dc_bits[agg]) break; *device_ptr = tm.dev.dc_bits[agg]; *num_elements = S * (int64_t)tm.dev.dc_words[agg]; return PB_OK;
-    case 4: *device_ptr = r->d_counters; *num_elements = PB_COUNTERS_PER_TABLE; return PB_OK;
-    case 5: *device_ptr = r->span_i64; *num_elements = r->span_i64_n; return PB_OK;
-    case 6: *device_ptr = r->span_f64; *num_elements = r->span_f64_n; return PB_OK;
-    case 7: *device_ptr = r->span_mm; *num_elements = r->span_mm_n; return PB_OK;
-    case 8: *device_ptr = r->block; *num_elements = r->block_bytes; return PB_OK;
-    default: break;
-  }
-  return fail(PB_ERR_INVALID, "no such device buffer (which=%d agg=%d)", which, agg);
+  // the table block is the one buffer handed out: its regions merge with four different operators and its fingerprint cell
+  // is checked against the number of ranks merged, which only the library's own merges record (pb_result_merge_gathered)
+  if (which != 8) return fail(PB_ERR_INVALID, "no such device buffer (which=%d agg=%d)", which, agg);
+  *device_ptr = r->block; *num_elements = r->block_bytes;
+  return PB_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -50,10 +50,19 @@ def test_reference_aggregation_expectations_on_the_device(dtype, base):
     r.free()
 
 
-def test_null_handling_fuzz_against_the_oracle():
-    """Random nullable columns (dictionary, raw, sorted, inverted), random filter trees with NOT / AND / OR / IS NULL, filtered
-    aggregations on top, several segments (one without any null vector), per segment and combined."""
-    native.init()
+FUZZ_QUERIES = [
+    "SELECT d, COUNT(*), COUNT(a), SUM(a), MIN(b), MAX(x), AVG(x) FROM t WHERE NOT (a > 2) GROUP BY d LIMIT 100",
+    "SELECT d, SUM(b), AVG(a), DISTINCTCOUNT(a) FROM t WHERE NOT (a IN (1, 2, 3) OR x < 0.5) AND s > 3 GROUP BY d LIMIT 100",
+    "SELECT COUNT(*), SUM(x), MIN(a), MAX(b), COUNT(b) FROM t WHERE a IS NULL OR NOT (b BETWEEN 100 AND 900)",
+    "SELECT d, COUNT(*), SUM(b) FILTER(WHERE NOT (a = 0)), MAX(x) FILTER(WHERE b > 500), COUNT(x) FROM t WHERE NOT (x > 4 AND a < 0) GROUP BY d LIMIT 100",
+    "SELECT COUNT(*), SUM(a), AVG(b) FROM t WHERE NOT (NOT (a < 0) AND NOT (x IS NULL)) AND s < 35",
+    "SELECT d, MIN(x), MAX(a) FROM t WHERE a <> 3 AND NOT (s = 7) GROUP BY d LIMIT 100",
+    "SELECT SUM(a), MIN(x), COUNT(a) FROM t WHERE a > 100",                     # nothing matches: every function is NULL, COUNT 0
+]
+
+
+def fuzz_segments():
+    """three segments of random nullable columns (dictionary, raw, sorted, inverted), one without any null vector"""
     rng = np.random.default_rng(21)
     segs = []
     for si, n in enumerate((20_011, 9_000, 14_500)):
@@ -72,17 +81,16 @@ def test_null_handling_fuzz_against_the_oracle():
                 with_nulls(build_column("x", DataType.DOUBLE, np.where(xn, 0.0, x)), xn),
                 with_nulls(build_column("s", DataType.INT, s), sn)]
         segs.append(make_segment(f"nh{si}", cols))
-    queries = [
-        "SELECT d, COUNT(*), COUNT(a), SUM(a), MIN(b), MAX(x), AVG(x) FROM t WHERE NOT (a > 2) GROUP BY d LIMIT 100",
-        "SELECT d, SUM(b), AVG(a), DISTINCTCOUNT(a) FROM t WHERE NOT (a IN (1, 2, 3) OR x < 0.5) AND s > 3 GROUP BY d LIMIT 100",
-        "SELECT COUNT(*), SUM(x), MIN(a), MAX(b), COUNT(b) FROM t WHERE a IS NULL OR NOT (b BETWEEN 100 AND 900)",
-        "SELECT d, COUNT(*), SUM(b) FILTER(WHERE NOT (a = 0)), MAX(x) FILTER(WHERE b > 500), COUNT(x) FROM t WHERE NOT (x > 4 AND a < 0) GROUP BY d LIMIT 100",
-        "SELECT COUNT(*), SUM(a), AVG(b) FROM t WHERE NOT (NOT (a < 0) AND NOT (x IS NULL)) AND s < 35",
-        "SELECT d, MIN(x), MAX(a) FROM t WHERE a <> 3 AND NOT (s = 7) GROUP BY d LIMIT 100",
-        "SELECT SUM(a), MIN(x), COUNT(a) FROM t WHERE a > 100",                     # nothing matches: every function is NULL, COUNT 0
-    ]
-    for sql in queries:
+    return segs
+
+
+def test_null_handling_fuzz_against_the_oracle():
+    """Random nullable columns (fuzz_segments), random filter trees with NOT / AND / OR / IS NULL, filtered aggregations on
+    top, several segments, per segment and combined."""
+    native.init()
+    segs = fuzz_segments()
+    for sql in FUZZ_QUERIES:
         # (a query with FILTER clauses of its own reports plain statistics under null handling, the reference its swim-lanes)
         check_query(segs, NH + sql, exact_float=False, check_stats="FILTER(" not in sql)
     # and the same statements without the option still run two-valued
-    check_query(segs, queries[0], exact_float=False)
+    check_query(segs, FUZZ_QUERIES[0], exact_float=False)
