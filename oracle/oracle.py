@@ -114,20 +114,21 @@ def lib():
         for f in (l.orc_lz4_block_decode, l.orc_snappy_block_decode):
             f.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
             f.restype = C.c_int64
-        l.orc_raw_forward_decompress.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64]
+        l.orc_raw_forward_decompress.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64]
         l.orc_raw_forward_decompress.restype = C.c_int64
         _lib = l
     return _lib
 
 
-def raw_forward_decompress(fwd: np.ndarray, width: int) -> np.ndarray:
-    """A chunk-compressed raw forward index rewritten as the equivalent PASS_THROUGH one (orc_raw_forward_decompress)."""
+def raw_forward_decompress(fwd: np.ndarray, width: int, num_docs: int = -1) -> np.ndarray:
+    """A chunk-compressed raw forward index rewritten as the equivalent PASS_THROUGH one (orc_raw_forward_decompress).
+    num_docs: the segment's doc count, which a version 1 index does not hold."""
     fwd = np.ascontiguousarray(fwd, dtype=np.uint8)
-    need = lib().orc_raw_forward_decompress(fwd.ctypes.data, fwd.size, width, None, 0)
+    need = lib().orc_raw_forward_decompress(fwd.ctypes.data, fwd.size, width, num_docs, None, 0)
     if need < 0:
         raise RuntimeError(lib().orc_last_error().decode())
     out = np.zeros(need, dtype=np.uint8)
-    if lib().orc_raw_forward_decompress(fwd.ctypes.data, fwd.size, width, out.ctypes.data, out.size) != need:
+    if lib().orc_raw_forward_decompress(fwd.ctypes.data, fwd.size, width, num_docs, out.ctypes.data, out.size) != need:
         raise RuntimeError(lib().orc_last_error().decode())
     return out
 
@@ -165,9 +166,9 @@ def marshal_segment(seg, m: _Marshalled, skip_inverted=()) -> OrcSegment:
         oc.bits_per_element = c.bits_per_element
         oc.dict_entry_bytes = c.dict_entry_bytes
         fwd = c.forward_index
-        if not c.has_dictionary and fwd.size >= 28 and int.from_bytes(fwd[0:4].tobytes(), "big") > 1 \
-                and int.from_bytes(fwd[20:24].tobytes(), "big") != 0:
-            fwd = m.hold(raw_forward_decompress(fwd, c.dict_entry_bytes))      # chunk codec -> plain values
+        version = int.from_bytes(fwd[0:4].tobytes(), "big") if not c.has_dictionary else 0
+        if not c.has_dictionary and (version == 1 or fwd.size >= 28 and version > 1 and int.from_bytes(fwd[20:24].tobytes(), "big") != 0):
+            fwd = m.hold(raw_forward_decompress(fwd, c.dict_entry_bytes, seg.num_docs))   # chunk codec -> plain values (v1: SNAPPY)
         oc.forward_index = fwd.ctypes.data
         oc.forward_index_len = fwd.size
         if c.dictionary is not None:

@@ -121,11 +121,12 @@ int64_t orc_snappy_block_decode(const uint8_t* in, int64_t in_len, uint8_t* out,
  * (SEGL/segment/index/readers/forward/BaseChunkForwardIndexReader.java:61-160, FixedByteChunkSVForwardIndexReader.java):
  * rewrites the index as the equivalent PASS_THROUGH one (same version, same chunking) so that the readers below see
  * plain values.  out == NULL returns the size needed; -1 = malformed / unsupported codec (ZSTANDARD, GZIP). */
-int64_t orc_raw_forward_decompress(const uint8_t* b, int64_t len, int32_t width, uint8_t* out, int64_t out_cap) {
+int64_t orc_raw_forward_decompress(const uint8_t* b, int64_t len, int32_t width, int32_t num_docs, uint8_t* out, int64_t out_cap) {
   if (len < 16) { set_err("raw forward index header"); return -1; }
   int32_t version = (int32_t)be32(b), num_chunks = (int32_t)be32(b + 4), docs_per_chunk = (int32_t)be32(b + 8);
   int32_t total_docs, codec, data_header_start;
   if (version > 1) { if (len < 28) { set_err("raw forward index header"); return -1; } total_docs = (int32_t)be32(b + 16); codec = (int32_t)be32(b + 20); data_header_start = (int32_t)be32(b + 24); }
+  else if (num_docs >= 0) { total_docs = num_docs; codec = 1; data_header_start = 16; }   /* version 1: four header ints, always SNAPPY */
   else { set_err("raw forward index v1 carries no doc count"); return -1; }
   int32_t entry = version <= 2 ? 4 : 8;
   int64_t raw_start = (int64_t)data_header_start + (int64_t)num_chunks * entry;
@@ -133,6 +134,7 @@ int64_t orc_raw_forward_decompress(const uint8_t* b, int64_t len, int32_t width,
   if (!out) return need;
   if (out_cap < need || raw_start > len) { set_err("raw forward index: buffer"); return -1; }
   memcpy(out, b, 16);
+  if (version == 1) { out[0] = out[1] = out[2] = 0; out[3] = 2; }   /* the same int offsets as version 2 */
   uint8_t hdr[12] = {0};
   hdr[0] = (uint8_t)(total_docs >> 24); hdr[1] = (uint8_t)(total_docs >> 16); hdr[2] = (uint8_t)(total_docs >> 8); hdr[3] = (uint8_t)total_docs;
   hdr[11] = 28;                                   /* compression 0, dataHeaderStart 28 */

@@ -151,7 +151,7 @@ int64_t orc_roaring_to_doc_ids(const uint8_t* blob, int64_t len, uint32_t* out, 
 /* chunk codecs of raw forward indexes (LZ4 block / raw Snappy) and the whole-index rewrite to PASS_THROUGH */
 int64_t orc_lz4_block_decode(const uint8_t* in, int64_t in_len, uint8_t* out, int64_t out_cap);
 int64_t orc_snappy_block_decode(const uint8_t* in, int64_t in_len, uint8_t* out, int64_t out_cap);
-int64_t orc_raw_forward_decompress(const uint8_t* fwd, int64_t len, int32_t width, uint8_t* out, int64_t out_cap);
+int64_t orc_raw_forward_decompress(const uint8_t* fwd, int64_t len, int32_t width, int32_t num_docs, uint8_t* out, int64_t out_cap);
 
 #ifdef __cplusplus
 }

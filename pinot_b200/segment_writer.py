@@ -219,32 +219,39 @@ COMPRESSION_LZ4_LENGTH_PREFIXED = 4
 _COMPRESSION_BY_NAME = {None: 0, "PASS_THROUGH": 0, "SNAPPY": 1, "LZ4": 3, "LZ4_LENGTH_PREFIXED": 4}
 
 
-def _compress_chunk(raw: bytes, compression: int) -> bytes:
+def _compress_chunk(raw: bytes, compression: int, block=None) -> bytes:
     """One chunk through the codec Pinot's ChunkCompressorFactory would use.  The compressors are pyarrow's bindings of the
     stock C libraries (liblz4 block format = lz4-java's fastCompressor output format; raw snappy = snappy-java's): this
-    module only frames them the way the reference's writers do."""
+    module only frames them the way the reference's writers do.  block: raw chunk -> LZ4 block or Snappy stream, in place
+    of the stock compressor (tests that emit chosen stream features)."""
     import pyarrow as pa
-    if compression == COMPRESSION_SNAPPY:
+    if block is not None:
+        z = block(raw)
+    elif compression == COMPRESSION_SNAPPY:
         return pa.Codec("snappy").compress(raw, asbytes=True)
-    z = pa.Codec("lz4_raw").compress(raw, asbytes=True)
+    else:
+        z = pa.Codec("lz4_raw").compress(raw, asbytes=True)
     if compression == COMPRESSION_LZ4_LENGTH_PREFIXED:        # lz4-java LZ4CompressorWithLength: little-endian decoded length
         return len(raw).to_bytes(4, "little") + z
     return z
 
 
 def _raw_forward_index(values: np.ndarray, data_type: DataType, compression=None, version: int = RAW_WRITER_VERSION,
-                       docs_per_chunk: int = RAW_DOCS_PER_CHUNK) -> np.ndarray:
+                       docs_per_chunk: int = RAW_DOCS_PER_CHUNK, block=None) -> np.ndarray:
     """BaseChunkForwardIndexWriter / FixedByteChunkForwardIndexWriter (SEGL/io/writer/impl/BaseChunkForwardIndexWriter.java:
     73-190): header of seven big-endian ints (version, numChunks, numDocsPerChunk, sizeOfEntry, totalDocs, compressionType,
-    dataHeaderStart), chunk offsets (int for version 2, long for 3 and 4), then the chunks, each compressed on its own;
-    the last chunk holds only the docs that are left."""
+    dataHeaderStart), chunk offsets (int for versions 1 and 2, long for 3 and 4), then the chunks, each compressed on its
+    own; the last chunk holds only the docs that are left.  Version 1 has only the first four header ints and no
+    compression field: its chunks are always SNAPPY.  block: see _compress_chunk."""
     comp = _COMPRESSION_BY_NAME[compression] if not isinstance(compression, int) else compression
-    assert version in (2, 3, 4)
+    assert version in (1, 2, 3, 4)
+    assert version > 1 or comp == COMPRESSION_SNAPPY, "version 1 chunks are SNAPPY"
     n = values.size
     width = _WIDTH[data_type]
     num_chunks = (n + docs_per_chunk - 1) // docs_per_chunk
-    off_dtype = ">i4" if version == 2 else ">i8"
-    header_size = 7 * 4 + num_chunks * (4 if version == 2 else 8)
+    off_dtype = ">i4" if version <= 2 else ">i8"
+    n_header_ints = 4 if version == 1 else 7
+    header_size = n_header_ints * 4 + num_chunks * (4 if version <= 2 else 8)
     header = np.empty(7, dtype=">i4")
     header[0] = version
     header[1] = num_chunks
@@ -253,6 +260,7 @@ def _raw_forward_index(values: np.ndarray, data_type: DataType, compression=None
     header[4] = n
     header[5] = comp
     header[6] = 7 * 4                              # dataHeaderStart
+    header = header[:n_header_ints]
     body = np.asarray(values).astype(_NP_BE[data_type]).tobytes()
     if comp == 0:
         offs = header_size + np.arange(num_chunks, dtype=np.int64) * (docs_per_chunk * width)
@@ -261,7 +269,7 @@ def _raw_forward_index(values: np.ndarray, data_type: DataType, compression=None
         chunks, offs, pos = [], [], header_size
         step = docs_per_chunk * width
         for k in range(num_chunks):
-            z = _compress_chunk(body[k * step:(k + 1) * step], comp)
+            z = _compress_chunk(body[k * step:(k + 1) * step], comp, block)
             offs.append(pos)
             chunks.append(z)
             pos += len(z)
@@ -296,8 +304,8 @@ def build_dict_column(name: str, data_type: DataType, dict_values_sorted: np.nda
 
 def build_column(name: str, data_type: DataType, values, dictionary: bool = True, inverted: bool = False,
                  run_optimize: bool = True, var_length_dictionary: bool = False, raw_compression=None,
-                 raw_version: int = RAW_WRITER_VERSION, raw_docs_per_chunk: int = RAW_DOCS_PER_CHUNK) -> ColumnIndex:
-    """Column from per-doc values (what SegmentIndexCreationDriverImpl does per column)."""
+                 raw_version: int = RAW_WRITER_VERSION, raw_docs_per_chunk: int = RAW_DOCS_PER_CHUNK, raw_block=None) -> ColumnIndex:
+    """Column from per-doc values (what SegmentIndexCreationDriverImpl does per column).  raw_block: see _compress_chunk."""
     if data_type == DataType.STRING:
         vals = np.array([v if isinstance(v, bytes) else str(v).encode("utf-8") for v in values], dtype=object)
         assert dictionary, "raw STRING columns are out of scope"
@@ -317,7 +325,7 @@ def build_column(name: str, data_type: DataType, values, dictionary: bool = True
     is_sorted = bool(n <= 1 or (vals[1:] >= vals[:-1]).all())
     return ColumnIndex(name=name, data_type=data_type, num_docs=n, has_dictionary=False, is_sorted=is_sorted,
                        cardinality=-1, bits_per_element=-1, dict_entry_bytes=_WIDTH[data_type],
-                       forward_index=_raw_forward_index(vals, data_type, raw_compression, raw_version, raw_docs_per_chunk),
+                       forward_index=_raw_forward_index(vals, data_type, raw_compression, raw_version, raw_docs_per_chunk, raw_block),
                        min_value=vals.min() if n else None, max_value=vals.max() if n else None)
 
 

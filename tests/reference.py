@@ -25,10 +25,12 @@ U = 2.0 ** -53                   # unit roundoff of double, round to nearest
 
 
 class Col(NamedTuple):
-    """values: int64 for INT / LONG, float64 for FLOAT (the float32 values widened) / DOUBLE, bytes ("S") for STRING"""
+    """values: int64 for INT / LONG, float64 for FLOAT (the float32 values widened) / DOUBLE, bytes ("S") for STRING;
+    nulls: the docs of the column's null-value vector (bool per doc), for IS [NOT] NULL; None: the column has none"""
     values: np.ndarray
     data_type: DataType
     has_dictionary: bool = True
+    nulls: Optional[np.ndarray] = None
 
 
 # ---- decoding a segment's columns (the writer's layouts) ----
@@ -109,6 +111,9 @@ def evaluate_sql(table, node):
         return ~evaluate_sql(table, node.child)
     c = table[node.column]
     v = c.values
+    if node.type in (PredicateType.IS_NULL, PredicateType.IS_NOT_NULL):
+        m = np.zeros(len(v), bool) if c.nulls is None else np.asarray(c.nulls, bool)
+        return ~m if node.type == PredicateType.IS_NOT_NULL else m.copy()
 
     def lit(s):
         if c.data_type == DataType.STRING:
@@ -127,6 +132,8 @@ def evaluate_sql(table, node):
             bits = v.astype(np.float64).view(np.int64)
             lits = [np.float32(x) if c.data_type == DataType.FLOAT else np.float64(x) for x in node.values]
             m = np.isin(bits, np.array([np.float64(x) for x in lits]).view(np.int64))
+        elif c.data_type in (DataType.INT, DataType.LONG):
+            m = np.isin(v, np.array([lit(x) for x in node.values], dtype=np.int64))
         else:
             m = np.logical_or.reduce([cmp(o.eq, lit(x)) for x in node.values])
         return ~m if t == PredicateType.NOT_IN else m
@@ -387,7 +394,12 @@ def concat(tables, columns=None) -> Dict[str, Col]:
     names = set(columns) if columns is not None else set(tables[0])
     for t in tables[1:]:
         names &= set(t)
-    return {c: Col(np.concatenate([t[c].values for t in tables]), tables[0][c].data_type, tables[0][c].has_dictionary) for c in names}
+    def nulls(c):
+        if all(t[c].nulls is None for t in tables):
+            return None
+        return np.concatenate([np.zeros(len(t[c].values), bool) if t[c].nulls is None else t[c].nulls for t in tables])
+    return {c: Col(np.concatenate([t[c].values for t in tables]), tables[0][c].data_type, tables[0][c].has_dictionary, nulls(c))
+            for c in names}
 
 
 # ---- comparison ----

@@ -40,8 +40,10 @@ def test_fixed_bit_stream_round_trip(w):   # PinotDataBitSetTest.testReadWriteIn
         assert l.orc_read_dict_id(padded.ctypes.data, w, i) == int(vals[i])
 
 
-def _roaring_decode_py(blob: bytes):
-    """RoaringBitmap portable format, decoded from the public spec alone (cookies 12346 / 12347)."""
+def _roaring_decode_py(blob: bytes, layout=None):
+    """RoaringBitmap portable format, decoded from the public spec alone (cookies 12346 / 12347).  layout: a dict that
+    receives the cookie, whether the blob has the offset header, and per container (key, cardinality, kind), kind one of
+    'array', 'bitmap', 'run'."""
     cookie = struct.unpack_from("<I", blob, 0)[0]
     pos = 4
     if cookie & 0xFFFF == 12347:
@@ -60,9 +62,14 @@ def _roaring_decode_py(blob: bytes):
     if has_offsets:
         pos += 4 * n
     out = []
+    if layout is not None:
+        layout.update(cookie=cookie & 0xFFFF, offsets=has_offsets, containers=[])
     for i, (key, card_m1) in enumerate(keys):
         card = card_m1 + 1
         base = key << 16
+        if layout is not None:
+            kind = "run" if run_flags[i // 8] >> (i % 8) & 1 else "bitmap" if card > 4096 else "array"
+            layout["containers"].append((key, card, kind))
         if run_flags[i // 8] >> (i % 8) & 1:
             nr = struct.unpack_from("<H", blob, pos)[0]
             pos += 2
