@@ -306,6 +306,21 @@ void pb_result_free(pb_result_handle r);
  * the block's layout fingerprint must be checked against the number of ranks merged. -------- */
 int pb_result_device_buffer(pb_result_handle r, int32_t which, int32_t agg, void** device_ptr, int64_t* num_elements);
 int pb_result_merge_gathered(pb_result_handle r, const void* gathered_device_ptr, int32_t n_ranks);
+/* -------- the same for a hash group table, whose groups are exchanged all-to-all: every rank keeps the groups whose key
+ * hashes to it.  pb_result_hash_partition packs this rank's groups by destination rank on the result's stream (wait for the
+ * stream before the exchange) and returns: the tuples for all n_ranks destinations, in rank order, as a device pointer the
+ * result owns (valid until its next partition or its free); counts[n_ranks] tuples per destination (host); the words (u64)
+ * per tuple; this rank's n_cells u64 counter cells (device); and the layout word (host), which covers what a tuple holds.
+ * PB_ERR_UNSUPPORTED: not a combined hash table, DISTINCTCOUNT, n_ranks > 64.
+ * Every rank then sends each destination its slice, all-gathers the counter cells (rank-major) and the layout words, and
+ * calls pb_result_hash_merge_received with the tuples it received concatenated in source-rank order (device), the gathered
+ * cells (device) and the layout words (host).  When a layout word differs it fails with PB_ERR_STATE before reading a tuple
+ * (the result can still be freed); otherwise it re-initialises the table, sized for what arrived, sums the cells and inserts
+ * the tuples.  Then pb_result_finalize hands back this rank's partition with the statistics of the whole query. -------- */
+int pb_result_hash_partition(pb_result_handle r, int32_t n_ranks, const void** tuples_device_ptr, int64_t* counts, int32_t* tuple_words,
+                             const void** cells_device_ptr, int32_t* n_cells, uint64_t* layout);
+int pb_result_hash_merge_received(pb_result_handle r, const void* tuples_device_ptr, int64_t n_tuples, const void* cells_device_ptr,
+                                  const uint64_t* layouts, int32_t n_ranks);
 int pb_result_finalize(pb_result_handle r);
 /* the CUDA stream (cudaStream_t) this result's work was issued on, and a host-side wait for it */
 void* pb_result_stream(pb_result_handle r);

@@ -1973,7 +1973,8 @@ __device__ __forceinline__ bool pb_slot_handed_back(const DevTable& t, uint64_t 
 // ------------------------------------------------------------------------------------------------
 // hash tables across ranks (SURVEY.md §8e: "partition tuples by hash(key) % nGPU, one all-to-all, local merge kernel"; the
 // reference merges by key in IndexedTable.upsert, CTR/data/table/IndexedTable.java:99-125).  A tuple is
-// [key words | row count | one u64 per aggregation (f64 sum bits / encoded min-max / filtered row count)].
+// [key words | row count | per aggregation: its f64 sum bits or encoded min-max (if it has one), then its own row count (if it
+// keeps one: COUNT / AVG under a FILTER clause, every function under one with enableNullHandling)].
 // ------------------------------------------------------------------------------------------------
 struct DevHashXfer {
   DevTable t;                                   // the local table
@@ -2022,8 +2023,11 @@ static __global__ void pb_hash_pack_kernel(const DevHashXfer X) {
     o[w++] = klo;
     if (X.t.key_words == 2) o[w++] = khi;
     o[w++] = c;
-    for (int a = 0; a < X.n_aggs; a++)
-      o[w++] = X.t.sum[a] ? (unsigned long long)__double_as_longlong(X.t.sum[a][i]) : X.t.mm[a] ? (unsigned long long)X.t.mm[a][i] : X.t.fcnt[a] ? X.t.fcnt[a][i] : 0ull;
+    for (int a = 0; a < X.n_aggs; a++) {
+      if (X.t.sum[a]) o[w++] = (unsigned long long)__double_as_longlong(X.t.sum[a][i]);
+      else if (X.t.mm[a]) o[w++] = (unsigned long long)X.t.mm[a][i];
+      if (X.t.fcnt[a]) o[w++] = X.t.fcnt[a][i];
+    }
   }
 }
 // received tuples -> this rank's (re-initialised) table
@@ -2038,10 +2042,9 @@ static __global__ void pb_hash_merge_kernel(const DevTable t, const unsigned lon
     if (slot == ~0ull) continue;                 // numGroupsLimit of the merged table (IndexedTable drops new keys past its limit too)
     pb_red_add_u64(&t.rowcnt[slot], c);
     for (int a = 0; a < n_aggs; a++) {
-      const unsigned long long v = p[w++];
-      if (t.sum[a]) pb_red_add_f64(&t.sum[a][slot], __longlong_as_double((long long)v));
-      else if (t.mm[a]) pb_red_min_s64(&t.mm[a][slot], (long long)v);
-      else if (t.fcnt[a]) pb_red_add_u64(&t.fcnt[a][slot], v);
+      if (t.sum[a]) pb_red_add_f64(&t.sum[a][slot], __longlong_as_double((long long)p[w++]));
+      else if (t.mm[a]) pb_red_min_s64(&t.mm[a][slot], (long long)p[w++]);
+      if (t.fcnt[a]) pb_red_add_u64(&t.fcnt[a][slot], p[w++]);
     }
   }
 }

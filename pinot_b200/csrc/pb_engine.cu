@@ -985,9 +985,11 @@ extern "C" int pb_segment_group_set_global_dictionary(pb_segment_group_handle g,
 // ------------------------------------------------------------------------------------------------
 struct HostArr {
   void* p = nullptr; size_t bytes = 0;
-  void alloc(size_t b) { bytes = b ? b : 8; p = pinned_alloc(bytes); }
+  void alloc(size_t b) { release(); bytes = b ? b : 8; p = pinned_alloc(bytes); }
   void release() { pinned_free(p, bytes); p = nullptr; }
 };
+
+struct DevBuf { void* p = nullptr; size_t cap = 0; };   // device memory of a result that grows on demand (stream-ordered)
 
 struct TableMeta {
   int mode = 0;
@@ -1078,6 +1080,11 @@ struct pb_result_s {
   Context* ctx = nullptr;
   std::vector<pb_result_s*> parts;          // multi-device group: the per-device results merged into this one (freed with it)
   std::vector<std::pair<int, int>> table_map;   // shell result of a multi-device per-segment query: table -> (part, table of the part)
+  // hash tables across ranks (comm_merge_hash): the table the aggregation fills, which the partition reads, and the larger
+  // table a merge receives into when this rank's share of the groups outgrows it (tables[0].dev is whichever holds the
+  // merged groups).  The buffers are kept for the next merge of a cached plan.
+  DevTable hash_local{}, hash_recv{};
+  DevBuf hx_ctl, hx_send, hx_gather, hx_recv, hx_table;
 };
 
 
@@ -1194,6 +1201,7 @@ static void destroy_result(pb_result_s* r) {
   release_segments(r);
   if (r->ctx) scratch_free(r->ctx, r->scratch, r->scratch_cap);
   for (void* p : r->dev_allocs) cudaFreeAsync(p, r->stream);
+  for (DevBuf* b : {&r->hx_ctl, &r->hx_send, &r->hx_gather, &r->hx_recv, &r->hx_table}) if (b->p) cudaFreeAsync(b->p, r->stream);
   for (auto& t : r->tables) {
     t.slots.release(); t.rows.release();
     for (auto* v : {&t.dbl, &t.lng, &t.key_ids, &t.key_vals, &t.dc_off, &t.dc_ids, &t.dc_vals}) for (auto& a : *v) a.release();
@@ -1471,6 +1479,7 @@ static int ensure_gather_buf(Context* ctx, size_t bytes, cudaStream_t st) {
 static int launch_merge(pb_result_s* r, const void* gathered, int n_rows, bool base_is_dst);
 static int launch_merge_rows(pb_result_s* r, const void* gathered, const DevMergePeers* peers, int n_rows, bool base_is_dst);
 static int comm_merge_hash(pb_result_s* r);
+static int prepare_finalize(pb_result_s* r);
 
 // All ranks call with the same query (PB_Q_ALL_RANKS): all-gather of the table blocks + one merge kernel, on the call's own
 // stream.  Every rank ends up with the merged table.
@@ -1644,6 +1653,7 @@ static int replay_plan(pb_result_s* r, const pb_query_desc* q) {
     if ((rc = enqueue_all(r, nullptr))) return rc;
     if (all_ranks && (rc = comm_merge(r))) return rc;
     if ((rc = enqueue_trim(r))) return rc;
+    if ((rc = prepare_finalize(r))) return rc;          // (again after a hash merge that changed the table: comm_merge_hash)
     if ((rc = enqueue_finalize(r))) return rc;
   }
   r->host_us[3] = now_us() - t1;
@@ -2062,6 +2072,7 @@ static int alloc_tables(Plan& P) {
     dt.othr = &sel->thr;
     r->d_sel.push_back(sel);
   }
+  if (r->table_mode == T_HASH) r->hash_local = r->tables[0].dev;
   return PB_OK;
 }
 
@@ -2486,10 +2497,18 @@ static int fill_counters_head(Plan& P) {
   // what must agree across ranks for the blocks to be mergeable element by element
   unsigned long long fp = 0xcbf29ce484222325ull;
   auto mix = [&](unsigned long long v) { fp ^= v; fp *= 0x100000001b3ull; fp ^= fp >> 29; };
-  mix((unsigned long long)r->block_bytes); mix((unsigned long long)r->block_sum_off); mix((unsigned long long)r->block_dc_off); mix((unsigned long long)r->block_mm_off);
-  mix((unsigned long long)r->table_mode); mix((unsigned long long)P.nG); mix((unsigned long long)P.nA); mix((unsigned long long)P.nF);
-  for (int a = 0; a < P.nA; a++) mix((unsigned long long)q->aggregations[a].op * 131 + P.dc_words[a]);
-  for (auto& tm : r->tables) { mix(tm.capacity); for (auto& f : tm.fields) mix(f.card); }
+  if (r->table_mode == T_HASH) {
+    // hash tables merge as tuples inserted by key (pb_hash_pack_kernel): what a tuple holds must agree, not the table's size,
+    // which follows each rank's doc count
+    mix((unsigned long long)r->table_mode); mix((unsigned long long)r->key_words); mix((unsigned long long)P.nG); mix((unsigned long long)P.nA);
+    for (int a = 0; a < P.nA; a++) mix((unsigned long long)q->aggregations[a].op * 131 + (has_fcnt(q, a) ? 1 : 0));
+    for (auto& tm : r->tables) for (auto& f : tm.fields) { mix((unsigned long long)f.width); mix(f.card); }
+  } else {
+    mix((unsigned long long)r->block_bytes); mix((unsigned long long)r->block_sum_off); mix((unsigned long long)r->block_dc_off); mix((unsigned long long)r->block_mm_off);
+    mix((unsigned long long)r->table_mode); mix((unsigned long long)P.nG); mix((unsigned long long)P.nA); mix((unsigned long long)P.nF);
+    for (int a = 0; a < P.nA; a++) mix((unsigned long long)q->aggregations[a].op * 131 + P.dc_words[a]);
+    for (auto& tm : r->tables) { mix(tm.capacity); for (auto& f : tm.fields) mix(f.card); }
+  }
   r->fingerprint = fp >> 8;                               // head room: n_ranks x fp must not wrap
   for (int t = 0; t < P.n_tables; t++) h_head[(size_t)t * PB_COUNTERS_PER_TABLE + 9] = r->fingerprint;
   return PB_OK;
@@ -3016,6 +3035,7 @@ static int enqueue_trim(pb_result_s* r) {
 // ---- result hand-back in three steps, so that a cached plan can re-enqueue step 2 without redoing step 1 ----
 // (1) pinned host arrays + the finalize descriptor of every table.  Very large tables are counted first (one extra pass
 //     and a synchronisation) so that the host arrays can be sized exactly; such plans are not cached.
+static const uint64_t SMALL_TABLE = 1ull << 20;
 static int prepare_finalize(pb_result_s* r) {
   pb_result_s::Replay& rp = r->rp;
   if (rp.fin_prepared) return PB_OK;
@@ -3026,7 +3046,6 @@ static int prepare_finalize(pb_result_s* r) {
   if (!r->h_counters.p) r->h_counters.alloc(8 * PB_COUNTERS_PER_TABLE * (size_t)nT);
   unsigned long long* hc = (unsigned long long*)r->h_counters.p;
   if (!hc) return fail(PB_ERR_OOM, "pinned host allocation failed");
-  const uint64_t SMALL_TABLE = 1ull << 20;
   bool any_big = false;
   for (int t = 0; t < nT; t++) {
     TableMeta& tm = r->tables[t];
@@ -3323,50 +3342,172 @@ extern "C" int32_t pb_result_plan_info(pb_result_handle r, int32_t* out, int32_t
 extern "C" void* pb_result_stream(pb_result_handle r) { return r ? (void*)r->stream : nullptr; }
 
 
-// Hash tables across ranks: every rank keeps the groups whose key hashes to it.  count -> exchange counts -> pack by
-// destination -> one grouped ncclSend/ncclRecv (all-to-all) -> re-initialise the local table -> insert what arrived.  The
-// statistics cells are summed over all ranks, so every rank reports the query's totals next to ITS partition of the groups;
-// the union of the partitions (disjoint by construction) is the merged table.
-static int comm_merge_hash(pb_result_s* r) {
-  const int n = g_comm.n_ranks;
-  if (n > 64) return fail(PB_ERR_UNSUPPORTED, "hash table merge over %d ranks (max 64)", n);
-  TableMeta& tm = r->tables[0];
-  const int nA = r->n_aggs;
-  for (int a = 0; a < nA; a++) if (r->agg_op[a] == PB_AGG_DISTINCTCOUNT) return fail(PB_ERR_UNSUPPORTED, "DISTINCTCOUNT in a hash group table is not merged across ranks");
+// Hash tables across ranks: every rank keeps the groups whose key hashes to it.  partition (count, then pack by
+// destination) -> exchange the tuples, the counter cells and the layout words -> merge received (re-initialise the table,
+// insert what arrived).  The statistics cells are summed over all ranks, so every rank reports the query's totals next to
+// ITS partition of the groups; the union of the partitions (disjoint by construction) is the merged table.
+static int grow(DevBuf& b, size_t bytes, cudaStream_t st) {
+  if (b.cap >= bytes) return PB_OK;
+  if (b.p) { CU(cudaFreeAsync(b.p, st)); b.p = nullptr; b.cap = 0; }
+  CU(cudaMallocAsync(&b.p, bytes, st));
+  b.cap = bytes;
+  return PB_OK;
+}
+static int hash_merge_supported(pb_result_s* r, int n_ranks) {
+  if (!r->combine || r->tables.size() != 1 || r->table_mode != T_HASH) return fail(PB_ERR_UNSUPPORTED, "a hash merge needs a combined (PB_Q_COMBINE) hash group table");
+  if (n_ranks < 1) return fail(PB_ERR_INVALID, "bad arguments");
+  if (n_ranks > 64) return fail(PB_ERR_UNSUPPORTED, "hash table merge over %d ranks (max 64)", n_ranks);
+  for (int a = 0; a < r->n_aggs; a++) if (r->agg_op[a] == PB_AGG_DISTINCTCOUNT) return fail(PB_ERR_UNSUPPORTED, "DISTINCTCOUNT in a hash group table is not merged across ranks");
+  return PB_OK;
+}
+// the layout words of all ranks, compared before a tuple moves: tuples of another width would be misread (and in a grouped
+// ncclSend / ncclRecv, mismatched sizes corrupt memory or hang)
+static int hash_layouts_agree(const pb_result_s* r, const uint64_t* layouts, int n_ranks) {
+  for (int k = 0; k < n_ranks; k++)
+    if (layouts[k] != r->fingerprint)
+      return fail(PB_ERR_STATE, "hash table merge: table layouts differ across ranks (rank %d: different query or global dictionaries)", k);
+  return PB_OK;
+}
+static int hash_tuple_words(const pb_result_s* r) {
+  const DevTable& t = r->hash_local;
+  int w = r->key_words + 1;
+  for (int a = 0; a < r->n_aggs; a++) w += (t.sum[a] || t.mm[a] ? 1 : 0) + (t.fcnt[a] ? 1 : 0);
+  return w;
+}
+static int hash_partition(pb_result_s* r, int n, const void** tuples, int64_t* counts, int32_t* tuple_words, const void** cells, int32_t* n_cells,
+                          uint64_t* layout) {
+  int rc = hash_merge_supported(r, n);
+  if (rc) return rc;
   cudaStream_t st = r->stream;
-  Context* ctx = r->ctx;
-  const int kw = r->key_words, T = kw + 1 + nA;
-  const int grid = (int)std::min<uint64_t>((pb_slots(tm.mode, tm.capacity) + 255) / 256, (uint64_t)ctx->num_sms * 8);
-  CU(cudaEventRecord(r->sset.ev[5], st));
-  // small control block: [counts n | cursors n | offsets n | all counts n*n | counter cells n*PB_COUNTERS_PER_TABLE]
-  const size_t ctl_words = (size_t)3 * n + (size_t)n * n + (size_t)n * PB_COUNTERS_PER_TABLE + 8;
-  unsigned long long* d_ctl = nullptr;
-  CU(cudaMallocAsync((void**)&d_ctl, 8 * ctl_words, st)); r->dev_allocs.push_back(d_ctl);
-  CU(cudaMemsetAsync(d_ctl, 0, 8 * ctl_words, st));
-  unsigned long long *d_counts = d_ctl, *d_cursors = d_ctl + n, *d_offsets = d_ctl + 2 * n, *d_all = d_ctl + 3 * n, *d_cells = d_ctl + 3 * n + (size_t)n * n;
+  const int T = hash_tuple_words(r);
+  const DevTable& t = r->hash_local;
+  const int grid = (int)std::min<uint64_t>((pb_slots(t.mode, t.capacity) + 255) / 256, (uint64_t)r->ctx->num_sms * 8);
+  if ((rc = grow(r->hx_ctl, 8 * 3 * (size_t)n, st))) return rc;
+  unsigned long long* d_ctl = (unsigned long long*)r->hx_ctl.p;      // [counts n | cursors n | offsets n]
+  CU(cudaMemsetAsync(d_ctl, 0, 8 * 3 * (size_t)n, st));
   DevHashXfer X; memset(&X, 0, sizeof X);
-  X.t = tm.dev; X.n_ranks = n; X.n_aggs = nA; X.tuple_words = T;
-  X.counts = d_counts; X.cursors = d_cursors; X.offsets = d_offsets;
+  X.t = t; X.n_ranks = n; X.n_aggs = r->n_aggs; X.tuple_words = T;
+  X.counts = d_ctl; X.cursors = d_ctl + n; X.offsets = d_ctl + 2 * n;
   pb_hash_count_kernel<<<grid, 256, 0, st>>>(X);
   r->launches++;
   CU(cudaGetLastError());
-  NC(g_comm.api.AllGather(d_counts, d_all, 8 * (size_t)n, ncclChar, g_comm.comm, st));
-  NC(g_comm.api.AllGather(r->d_counters, d_cells, 8 * (size_t)PB_COUNTERS_PER_TABLE, ncclChar, g_comm.comm, st));
-  std::vector<unsigned long long> all((size_t)n * n);
-  CU(cudaMemcpyAsync(all.data(), d_all, 8 * all.size(), cudaMemcpyDeviceToHost, st));
+  std::vector<unsigned long long> cnt((size_t)n), off((size_t)n + 1, 0);
+  CU(cudaMemcpyAsync(cnt.data(), d_ctl, 8 * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  const int me = g_comm.rank;
-  std::vector<unsigned long long> soff((size_t)n + 1, 0), roff((size_t)n + 1, 0);
-  for (int k = 0; k < n; k++) { soff[k + 1] = soff[k] + all[(size_t)me * n + k]; roff[k + 1] = roff[k] + all[(size_t)k * n + me]; }
-  const uint64_t n_send = soff[n], n_recv = roff[n];
-  unsigned long long *d_send = nullptr, *d_recv = nullptr;
-  CU(cudaMallocAsync((void**)&d_send, 8 * (size_t)T * std::max<uint64_t>(n_send, 1), st)); r->dev_allocs.push_back(d_send);
-  CU(cudaMallocAsync((void**)&d_recv, 8 * (size_t)T * std::max<uint64_t>(n_recv, 1), st)); r->dev_allocs.push_back(d_recv);
-  CU(cudaMemcpyAsync(d_offsets, soff.data(), 8 * (size_t)n, cudaMemcpyHostToDevice, st));
-  X.out = d_send;
+  for (int k = 0; k < n; k++) { off[k + 1] = off[k] + cnt[k]; counts[k] = (int64_t)cnt[k]; }
+  if ((rc = grow(r->hx_send, 8 * (size_t)T * std::max<uint64_t>(off[n], 1), st))) return rc;
+  CU(cudaMemcpyAsync(d_ctl + 2 * n, off.data(), 8 * (size_t)n, cudaMemcpyHostToDevice, st));
+  X.out = (unsigned long long*)r->hx_send.p;
   pb_hash_pack_kernel<<<grid, 256, 0, st>>>(X);
   r->launches++;
   CU(cudaGetLastError());
+  *tuples = r->hx_send.p; *tuple_words = T; *cells = r->d_counters; *n_cells = PB_COUNTERS_PER_TABLE; *layout = r->fingerprint;
+  return PB_OK;
+}
+// The table the merged partition goes into, re-initialised: the aggregation's own table when it has the slots for what
+// arrived (2 x min(numGroupsLimit, tuples received), like a table sized from its docs), else the receive table, grown to that.
+static int hash_receive_table(pb_result_s* r, uint64_t n_recv, DevTable* out) {
+  cudaStream_t st = r->stream;
+  const DevTable& L = r->hash_local;
+  const uint64_t want = std::min<uint64_t>(L.num_groups_limit, std::max<uint64_t>(n_recv, 1));
+  uint64_t cap = 1024;
+  while (cap < 2 * want) cap <<= 1;
+  if (cap <= L.capacity) {
+    // (the counter cells head the zero region: they stay)
+    const uint64_t skip16 = (((uint64_t)PB_COUNTERS_PER_TABLE * 8 + 255) & ~(uint64_t)255) / 16;
+    pb_init_tables_kernel<<<r->init.grid, 256, 0, st>>>(r->init.zero + skip16, r->init.zn - skip16, r->init.ff, r->init.fn, r->init.mm, r->init.mn,
+                                                         nullptr, 0, nullptr, 0);
+    r->launches++;
+    *out = L;
+    return PB_OK;
+  }
+  // (kept from an earlier merge when it is large enough)
+  DevTable& R = r->hash_recv;
+  if (R.capacity < cap) R.capacity = cap;
+  const uint64_t S2 = (pb_slots(T_HASH, R.capacity) + 1) & ~(uint64_t)1;     // every region a multiple of 16 bytes (CAS.128 on the keys)
+  int n_zero = 1, n_mm = 0;
+  for (int a = 0; a < r->n_aggs; a++) n_zero += (L.sum[a] ? 1 : 0) + (L.fcnt[a] ? 1 : 0), n_mm += L.mm[a] ? 1 : 0;
+  const uint64_t zw = n_zero * S2, mw = n_mm * S2, fw = (uint64_t)L.key_words * S2, ow = L.okey ? S2 : 0;
+  // [zero: row counts, own row counts, sums | min-max | 0xFF: keys | order keys]
+  int rc = grow(r->hx_table, 8 * (zw + mw + fw + ow), st);
+  if (rc) return rc;
+  unsigned long long* p = (unsigned long long*)r->hx_table.p;
+  const uint64_t capacity = R.capacity;
+  R = L;                                                // counter cells, numGroupsLimit, trim state: the local table's
+  R.capacity = capacity;
+  R.rowcnt = p; p += S2;
+  for (int a = 0; a < r->n_aggs; a++) {
+    if (L.fcnt[a]) { R.fcnt[a] = p; p += S2; }
+    if (L.sum[a]) { R.sum[a] = (double*)p; p += S2; }
+  }
+  uint4* mm = (uint4*)p;
+  for (int a = 0; a < r->n_aggs; a++) if (L.mm[a]) { R.mm[a] = (long long*)p; p += S2; }
+  R.hkeys = p; p += fw;
+  if (L.okey) R.okey = p;
+  const uint64_t mx = std::max(zw, std::max(mw, fw)) / 2;
+  const int grid = (int)std::max<uint64_t>(std::min<uint64_t>((mx + 255) / 256, (uint64_t)r->ctx->num_sms * 8), 1);
+  pb_init_tables_kernel<<<grid, 256, 0, st>>>((uint4*)R.rowcnt, zw / 2, (uint4*)R.hkeys, fw / 2, mm, mw / 2, nullptr, 0, nullptr, 0);
+  r->launches++;
+  *out = R;
+  return PB_OK;
+}
+static int hash_merge_received(pb_result_s* r, const void* tuples, uint64_t n_recv, const void* cells, const uint64_t* layouts, int n) {
+  int rc = hash_merge_supported(r, n);
+  if (rc || (rc = hash_layouts_agree(r, layouts, n))) return rc;
+  cudaStream_t st = r->stream;
+  TableMeta& tm = r->tables[0];
+  DevTable t;
+  if ((rc = hash_receive_table(r, n_recv, &t))) return rc;
+  CU(cudaMemsetAsync(r->d_counters, 0, 8, st));     // num_groups: recounted by the inserts
+  pb_sum_counters_kernel<<<1, 32, 0, st>>>(r->d_counters, (const unsigned long long*)cells, n, PB_COUNTERS_PER_TABLE);
+  r->launches++;
+  if (n_recv) {
+    DevTable ins = t;
+    ins.limit_active = (uint64_t)t.num_groups_limit < n_recv ? 1u : 0u;     // groups <= tuples: see DevTable::limit_active
+    const int mgrid = (int)std::min<uint64_t>((n_recv + 255) / 256, (uint64_t)r->ctx->num_sms * 8);
+    pb_hash_merge_kernel<<<mgrid, 256, 0, st>>>(ins, (const unsigned long long*)tuples, n_recv, r->key_words, r->n_aggs, hash_tuple_words(r));
+    r->launches++;
+  }
+  CU(cudaGetLastError());
+  // the hand-back reads the table the merge filled: descriptors built for another table, or sized by a count of the groups
+  // of an earlier run, are built again
+  if (r->rp.fin_prepared && (r->rp.fin[0].t.rowcnt != t.rowcnt || r->rp.fin[0].t.capacity != t.capacity || pb_slots(T_HASH, t.capacity) > SMALL_TABLE)) r->rp.fin_prepared = false;
+  tm.dev = t; tm.capacity = t.capacity;
+  r->merged_ranks *= n;
+  return PB_OK;
+}
+// (the NCCL path of PB_Q_ALL_RANKS: the same two steps, with the exchange in between)
+static int comm_merge_hash(pb_result_s* r) {
+  const int n = g_comm.n_ranks, me = g_comm.rank;
+  cudaStream_t st = r->stream;
+  CU(cudaEventRecord(r->sset.ev[5], st));
+  const void *send = nullptr, *cells = nullptr;
+  std::vector<int64_t> counts((size_t)n);
+  int32_t T = 0, n_cells = 0;
+  uint64_t layout = 0;
+  int rc = hash_partition(r, n, &send, counts.data(), &T, &cells, &n_cells, &layout);
+  if (rc) return rc;
+  // all-gather [tuples per destination | layout word] of every rank and the counter cells
+  const size_t w = (size_t)n + 1;
+  if ((rc = grow(r->hx_gather, 8 * (w + (size_t)n * w + (size_t)n * n_cells), st))) return rc;
+  unsigned long long *d_mine = (unsigned long long*)r->hx_gather.p, *d_all = d_mine + w, *d_cells = d_all + (size_t)n * w;
+  std::vector<unsigned long long> mine(w), all((size_t)n * w);
+  for (int k = 0; k < n; k++) mine[k] = (unsigned long long)counts[k];
+  mine[n] = layout;
+  CU(cudaMemcpyAsync(d_mine, mine.data(), 8 * w, cudaMemcpyHostToDevice, st));
+  NC(g_comm.api.AllGather(d_mine, d_all, 8 * w, ncclChar, g_comm.comm, st));
+  NC(g_comm.api.AllGather(cells, d_cells, 8 * (size_t)n_cells, ncclChar, g_comm.comm, st));
+  CU(cudaMemcpyAsync(all.data(), d_all, 8 * all.size(), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  std::vector<uint64_t> layouts((size_t)n);
+  for (int k = 0; k < n; k++) layouts[k] = all[(size_t)k * w + n];
+  if ((rc = hash_layouts_agree(r, layouts.data(), n))) return rc;       // every rank sees every word: all of them refuse
+  std::vector<unsigned long long> soff((size_t)n + 1, 0), roff((size_t)n + 1, 0);
+  for (int k = 0; k < n; k++) { soff[k + 1] = soff[k] + all[(size_t)me * w + k]; roff[k + 1] = roff[k] + all[(size_t)k * w + me]; }
+  const uint64_t n_recv = roff[n];
+  if ((rc = grow(r->hx_recv, 8 * (size_t)T * std::max<uint64_t>(n_recv, 1), st))) return rc;
+  const unsigned long long* d_send = (const unsigned long long*)send;
+  unsigned long long* d_recv = (unsigned long long*)r->hx_recv.p;
   NC(g_comm.api.GroupStart());
   for (int k = 0; k < n; k++) {
     const size_t sb = 8 * (size_t)T * (size_t)(soff[k + 1] - soff[k]), rb = 8 * (size_t)T * (size_t)(roff[k + 1] - roff[k]);
@@ -3374,25 +3515,22 @@ static int comm_merge_hash(pb_result_s* r) {
     if (rb) NC(g_comm.api.Recv(d_recv + (size_t)T * roff[k], rb, ncclChar, k, g_comm.comm, st));
   }
   NC(g_comm.api.GroupEnd());
-  // the local table starts over (its rows all travelled, this rank's own share included); the counters stay
-  {
-    const uint64_t skip16 = (((uint64_t)PB_COUNTERS_PER_TABLE * 8 + 255) & ~(uint64_t)255) / 16;      // counter cells of the one table
-    pb_init_tables_kernel<<<r->init.grid, 256, 0, st>>>(r->init.zero + skip16, r->init.zn - skip16, r->init.ff, r->init.fn, r->init.mm, r->init.mn,
-                                                         nullptr, 0, nullptr, 0);
-    CU(cudaMemsetAsync(r->d_counters, 0, 8, st));     // num_groups: recounted by the inserts
-    pb_sum_counters_kernel<<<1, 32, 0, st>>>(r->d_counters, d_cells, n, PB_COUNTERS_PER_TABLE);
-    r->launches += 2;
-  }
-  if (n_recv) {
-    const int mgrid = (int)std::min<uint64_t>((n_recv + 255) / 256, (uint64_t)ctx->num_sms * 8);
-    pb_hash_merge_kernel<<<mgrid, 256, 0, st>>>(tm.dev, d_recv, n_recv, kw, nA, T);
-    r->launches++;
-  }
-  CU(cudaGetLastError());
+  if ((rc = hash_merge_received(r, d_recv, n_recv, d_cells, layouts.data(), n))) return rc;
   CU(cudaEventRecord(r->sset.ev[6], st));
   r->comm_timed = true;
-  r->merged_ranks *= n;
   return PB_OK;
+}
+extern "C" int pb_result_hash_partition(pb_result_handle r, int32_t n_ranks, const void** tuples, int64_t* counts, int32_t* tuple_words,
+                                        const void** cells, int32_t* n_cells, uint64_t* layout) {
+  if (!r || !tuples || !counts || !tuple_words || !cells || !n_cells || !layout) return fail(PB_ERR_INVALID, "null argument");
+  DeviceGuard dg(r->ctx);
+  return hash_partition(r, n_ranks, tuples, counts, tuple_words, cells, n_cells, layout);
+}
+extern "C" int pb_result_hash_merge_received(pb_result_handle r, const void* tuples, int64_t n_tuples, const void* cells, const uint64_t* layouts,
+                                             int32_t n_ranks) {
+  if (!r || n_tuples < 0 || (n_tuples > 0 && !tuples) || !cells || !layouts) return fail(PB_ERR_INVALID, "bad arguments");
+  DeviceGuard dg(r->ctx);
+  return hash_merge_received(r, tuples, (uint64_t)n_tuples, cells, layouts, n_ranks);
 }
 static int launch_merge_rows(pb_result_s* r, const void* gathered, const DevMergePeers* peers, int n_rows, bool base_is_dst) {
   if (!r->combine || r->tables.size() != 1 || r->table_mode == T_HASH) return fail(PB_ERR_UNSUPPORTED, "merge needs a combined dense / keyless result");

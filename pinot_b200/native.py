@@ -162,6 +162,9 @@ def lib():
     l.pb_result_stream.restype = C.c_void_p
     l.pb_result_wait.argtypes = [C.c_void_p]
     l.pb_result_merge_gathered.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+    l.pb_result_hash_partition.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int32),
+                                           C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_uint64)]
+    l.pb_result_hash_merge_received.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(C.c_uint64), C.c_int32]
     l.pb_result_phase_ms.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     l.pb_result_host_timing.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
     l.pb_host_register.argtypes = [C.c_void_p, C.c_size_t]
@@ -447,6 +450,24 @@ class Result:
 
     def merge_gathered(self, gathered_ptr: int, n_ranks: int):
         _check(lib().pb_result_merge_gathered(self._rh, gathered_ptr, n_ranks))
+
+    def hash_partition(self, n_ranks: int):
+        """This rank's groups of a deferred hash table packed by destination rank (pb_result_hash_partition), enqueued on
+        the result's stream: (tuples device pointer, tuples per destination, u64 words per tuple, counter cells device
+        pointer, number of cells, layout word)"""
+        tuples, cells, words, n_cells, layout = C.c_void_p(), C.c_void_p(), C.c_int32(), C.c_int32(), C.c_uint64()
+        counts = (C.c_int64 * max(n_ranks, 1))()
+        _check(lib().pb_result_hash_partition(self._rh, n_ranks, C.byref(tuples), counts, C.byref(words), C.byref(cells), C.byref(n_cells),
+                                              C.byref(layout)))
+        return tuples.value, list(counts)[:n_ranks], words.value, cells.value, n_cells.value, layout.value
+
+    def hash_merge_received(self, tuples_ptr: int, n_tuples: int, cells_ptr: int, layouts, n_ranks: int):
+        """merge the tuples this rank received (source-rank order) with the counter cells (rank-major) and layout words of
+        all ranks (pb_result_hash_merge_received)"""
+        if len(layouts) < n_ranks:
+            raise ValueError(f"{len(layouts)} layout words for {n_ranks} ranks")
+        words = (C.c_uint64 * max(len(layouts), 1))(*layouts)
+        _check(lib().pb_result_hash_merge_received(self._rh, tuples_ptr, n_tuples, cells_ptr, words, n_ranks))
 
     def stream(self) -> int:
         return lib().pb_result_stream(self._rh) or 0

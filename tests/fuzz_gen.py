@@ -220,3 +220,22 @@ def make_shaped_query(rng, src: Dict[str, Col]) -> str:
     ngl = int(rng.choice([1, 2, 5, 20, 300])) if rng.random() < 0.5 else 100000000
     return f"SET numGroupsLimit = {ngl}; {opts}SELECT {', '.join(aggs)} FROM t{where_clause(rng, src)} GROUP BY {', '.join(keys)} " \
            f"ORDER BY {ob} {'DESC' if rng.random() < 0.5 else 'ASC'} LIMIT {limit}"
+
+
+HASH_KEY_SETS = [["rki", "rkj"], ["rkl"],                     # raw keys, one key word
+                 ["rki", "rkj", "k2"], ["rkl", "rki", "k3", "kstr"]]     # two key words
+
+
+def make_hash_query(rng, src: Dict[str, Col], wide_card: int = WIDE) -> str:
+    """A query whose group table is a hash table (the hash key sets of KEY_SETS; kwa, kwb when kwb has 4097 values): COUNT /
+    SUM / MIN / MAX / AVG, about 30 % of them under a FILTER clause.  Its own rng stream (make_query's seeds and coverage stay
+    as they are)."""
+    key_sets = HASH_KEY_SETS + ([["kwa", "kwb"]] if wide_card > WIDE else [])
+    keys = key_sets[int(rng.integers(0, len(key_sets)))]
+    aggs = []
+    for _ in range(int(rng.integers(1, 6))):
+        op = str(rng.choice(["COUNT", "SUM", "MIN", "MAX", "AVG"]))
+        col = "*" if op == "COUNT" else str(rng.choice(MINMAX_COLS if op in ("MIN", "MAX") else SUM_COLS))
+        flt = f" FILTER(WHERE {_expr(rng, src, 1)})" if rng.random() < 0.3 else ""
+        aggs.append(f"{op}({col}){flt}")
+    return f"SET numGroupsLimit = 100000000; SELECT {', '.join(aggs)} FROM t{where_clause(rng, src)} GROUP BY {', '.join(keys)} LIMIT 100000000"

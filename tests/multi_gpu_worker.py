@@ -91,8 +91,11 @@ def run_ranks(rank, world, xdir):
             check(f"rank {rank}: {name} (pass {rep})", res, exp, orc, q, exact, len(all_segs))   # EVERY rank holds the merged table
             assert res.comm_ms() > 0
             res.free()
-    # a query whose group table is a hash table (raw LONG key)
-    q = parse_sql("SET numGroupsLimit = 10000000; SELECT k0, SUM(m0), COUNT(*) FROM t GROUP BY k0 LIMIT 10000000")
+    # a query whose group table is a hash table (raw LONG key); the filtered AVG keeps its own row count, which travels in
+    # the tuples next to its sum
+    d3 = all_segs[0].columns["c3"].dictionary_values()
+    q = parse_sql(f"SET numGroupsLimit = 10000000; SELECT k0, SUM(m0), COUNT(*), AVG(m0) FILTER(WHERE c3 < {int(d3[len(d3) // 3])}) FROM t "
+                  "GROUP BY k0 LIMIT 10000000")
     exp, orc = expected(all_segs, q)
     res = native.execute(group, q, flags)
     # hash tables are merged by a hash-partitioned all-to-all: every rank holds the groups whose key hashes to it (disjoint

@@ -7,8 +7,8 @@ rank-major into one buffer: what an all-gather would deliver.  pb_result_merge_g
 pb_merge_blocks_kernel, the real local-to-global remaps and the real hand-back over a merged table, and the result is judged by
 tests/reference.py over all segments of all ranks.
 
-Not covered here: NCCL itself (comm_merge's collectives), the hash-partitioned all-to-all of hash tables
-(pb_hash_count_kernel / pb_hash_pack_kernel), and the pointer plumbing of the NVLink peer merge.
+Not covered here: NCCL itself (comm_merge's collectives) and the pointer plumbing of the NVLink peer merge.  The
+hash-partitioned all-to-all of hash tables is held to the reference the same way in tests/test_gpu_hash_merge.py.
 
 PB_FUZZ_SEEDS="1,3" narrows the fuzz seeds."""
 import contextlib
