@@ -69,6 +69,9 @@ struct Context {
   uint64_t lru_clock = 0;
   uint64_t evictions = 0;
   std::vector<struct pb_segment_s*> segments; // every live segment staged on this device (eviction candidates)
+  // held by an eviction pass across its walk over a copy of `segments`, and by pb_segment_release around its erase and
+  // delete.  Lock order: evict_mu, then a segment's mu, then mu.
+  std::mutex evict_mu;
   // cross-rank merge (pb_comm_init): receive buffer of the table all-gather, grown on demand
   void* gather_buf = nullptr; size_t gather_cap = 0;
 };
@@ -604,20 +607,21 @@ static void drop_device_copies(pb_segment_s* s) {     // under s->mu, inflight =
 static void enforce_cache_limit(Context* ctx) {
   const size_t limit = g_all.hbm_cache_bytes;
   if (!limit) return;
+  auto within = [&]() { std::lock_guard<std::mutex> lk(ctx->mu); return (size_t)std::max<int64_t>(ctx->staged_bytes, 0) <= limit; };
+  if (within()) return;
+  // the candidates are a copy of ctx->segments: pb_segment_release waits for evict_mu, so none of them is deleted under us
+  std::lock_guard<std::mutex> el(ctx->evict_mu);
   std::vector<pb_segment_s*> cand;
   {
     std::lock_guard<std::mutex> lk(ctx->mu);
-    if ((size_t)std::max<int64_t>(ctx->staged_bytes, 0) <= limit) return;
     cand = ctx->segments;
   }
   std::sort(cand.begin(), cand.end(), [](const pb_segment_s* a, const pb_segment_s* b) { return a->last_used < b->last_used; });
   for (pb_segment_s* s : cand) {
-    {
-      std::lock_guard<std::mutex> lk(ctx->mu);
-      if ((size_t)std::max<int64_t>(ctx->staged_bytes, 0) <= limit) return;
-    }
+    if (within()) return;
     std::unique_lock<std::mutex> sl(s->mu, std::try_to_lock);
-    if (!sl.owns_lock() || s->inflight > 0 || s->device_bytes == 0) continue;
+    // (stage_dirty: copies enqueued without a staging event behind them yet -- they may still be reading the pinned sources)
+    if (!sl.owns_lock() || s->inflight > 0 || s->device_bytes == 0 || s->stage_dirty) continue;
     if (s->staged_pending) {
       if (cudaEventQuery(s->staged_ev) != cudaSuccess) { cudaGetLastError(); continue; }
       s->staged_pending = false;
@@ -694,6 +698,9 @@ static const RowGroup* row_group_for(pb_segment_s* s, std::vector<std::pair<int,
 extern "C" int pb_segment_release(pb_segment_handle s) {
   if (!s) return PB_OK;
   DeviceGuard dg(s->ctx);
+  // an eviction pass in progress holds a copy of ctx->segments: the segment leaves the list and dies only after it
+  std::unique_lock<std::mutex> el;
+  if (s->ctx) el = std::unique_lock<std::mutex>(s->ctx->evict_mu);
   if (s->ctx) {
     std::lock_guard<std::mutex> lk(s->ctx->mu);
     auto& v = s->ctx->segments;
@@ -1153,9 +1160,7 @@ static void plan_register(pb_group_s* g, pb_result_s* r, std::string&& sig) {
     std::lock_guard<std::mutex> lk(g_plan_mu);
     r->rp.sig = std::move(sig); r->rp.owner = g; r->rp.busy = true;
     r->rp.host_sig = g_pending_host_key;
-    r->rp.dict_version = g->dict_version;
-    r->rp.seg_epochs.clear();
-    for (auto* sg : g->segs) r->rp.seg_epochs.push_back(sg->epoch);
+    r->rp.dict_version = g->dict_version;       // (rp.seg_epochs: read by stage_segment while the call had them pinned)
     g->plans.push_back(r);
     for (size_t i = 0; g->plans.size() > PB_MAX_PLANS_PER_GROUP && i < g->plans.size();) {      // oldest idle plans go first
       if (!g->plans[i]->rp.busy) { evict.push_back(g->plans[i]); g->plans[i]->rp.owner = nullptr; g->plans.erase(g->plans.begin() + (long)i); }
@@ -1587,13 +1592,41 @@ static int enqueue_all(pb_result_s* r, const std::vector<cudaEvent_t>* seg_wait)
 }
 
 
+// A parked plan whose segments changed between the lookup and the pin (another call evicted one, or replaced one of its
+// row groups): it is taken out of its group and destroyed, and the caller plans the query afresh
+static void plan_retire(pb_result_s* r) {
+  {
+    std::lock_guard<std::mutex> lk(g_plan_mu);
+    if (pb_group_s* g = r->rp.owner) g->plans.erase(std::remove(g->plans.begin(), g->plans.end(), r), g->plans.end());
+    r->rp.owner = nullptr;
+  }
+  destroy_result(r);
+}
+#define PB_REPLAY_STALE 1            // replay_plan: the plan was retired, nothing ran
+
 // Run a cached plan again: pin the segments, re-enqueue the kernels (one graph launch from the second reuse on), hand back.
+// The lookup compared the segments' epochs without pinning them: they are compared again under each pin, since an eviction
+// in between would leave the plan pointing into freed memory.  PB_REPLAY_STALE: the plan was retired instead.
 static int replay_plan(pb_result_s* r, const pb_query_desc* q) {
   pb_result_s::Replay& rp = r->rp;
   pb_group_s* g = r->group;
   Context* ctx = r->ctx;
   cudaStream_t st = r->stream;
   const double t0 = now_us();
+  bool same = rp.seg_epochs.size() == g->segs.size();
+  for (size_t si = 0; same && si < g->segs.size(); si++) {
+    pb_segment_s* sg = g->segs[si];
+    std::lock_guard<std::mutex> lk(sg->mu);
+    sg->inflight++; r->pinned_segments = (int)si + 1;
+    same = sg->epoch == rp.seg_epochs[si];
+    std::lock_guard<std::mutex> lk2(ctx->mu);
+    sg->last_used = ++ctx->lru_clock;
+  }
+  if (!same) {
+    release_segments(r);
+    plan_retire(r);
+    return PB_REPLAY_STALE;
+  }
   r->finalized = false; r->launches = 0; r->comm_timed = false; r->comm_ms = 0; r->merged_ranks = 1;
   for (int i = 0; i < 8; i++) r->host_us[i] = 0;
   for (auto& tm : r->tables) {
@@ -1601,13 +1634,6 @@ static int replay_plan(pb_result_s* r, const pb_query_desc* q) {
     for (auto& a : tm.dc_off) a.release();        // DISTINCTCOUNT value sets of the previous run (materialised on demand)
     for (auto& a : tm.dc_ids) a.release();
     for (auto& a : tm.dc_vals) a.release();
-  }
-  for (size_t si = 0; si < g->segs.size(); si++) {
-    pb_segment_s* sg = g->segs[si];
-    std::lock_guard<std::mutex> lk(sg->mu);
-    sg->inflight++; r->pinned_segments = (int)si + 1;
-    std::lock_guard<std::mutex> lk2(ctx->mu);
-    sg->last_used = ++ctx->lru_clock;
   }
   int rc = PB_OK;
   const bool all_ranks = (q->flags & PB_Q_ALL_RANKS) != 0;
@@ -1781,17 +1807,12 @@ static int pick_row_group(Plan& P, int si) {
   return PB_OK;
 }
 
-// Pin segment si, resolve the columns the query names and stage what its kernels read, build its row group, and record
-// the staging event its kernels must wait for
-static int stage_segment(Plan& P, int si) {
+// Resolve the columns the query names on segment si and stage what its kernels read, then build its row group.  Under s->mu.
+static int stage_segment_columns(Plan& P, int si) {
   int rc;
   pb_segment_s* s = P.g->segs[si];
   const pb_query_desc* q = P.q;
-  Context* ctx = P.ctx;
-  cudaStream_t cs = ctx->copy_stream;
-  std::lock_guard<std::mutex> lk(s->mu);
-  s->inflight++; P.r->pinned_segments = si + 1;
-  { std::lock_guard<std::mutex> lk2(ctx->mu); s->last_used = ++ctx->lru_clock; }
+  cudaStream_t cs = P.ctx->copy_stream;
   // (PB_IN_PLACE_COST overrides the cost of an in-place value; 0 = always gather: used by the tests to reach every code path.)
   const double sel = P.in_place ? estimate_selectivity(s, P.sqs[si]) : 1.0;
   double gather_cost = 56.0;
@@ -1826,7 +1847,20 @@ static int stage_segment(Plan& P, int si) {
     if (sq.agg_filter_nodes[f] < 0 || sq.agg_filter_nodes[f] > PB_MAX_AF_NODES) return fail(PB_ERR_UNSUPPORTED, "FILTER clause %d has %d nodes (max %d)", f, sq.agg_filter_nodes[f], PB_MAX_AF_NODES);
     if ((rc = stage_filter_columns(s, sq.agg_filters[f], sq.agg_filter_nodes[f], f, cs, [&](int, const Column& c) { return gather_ok(c); }))) return rc;
   }
-  if ((rc = pick_row_group(P, si))) return rc;
+  return pick_row_group(P, si);
+}
+
+// Pin segment si, stage it (stage_segment_columns), account its new bytes and record the staging event its kernels must
+// wait for.  A refused call (a column that does not stage) keeps what its earlier columns staged: those bytes are accounted
+// and their copies are marked by the event too, so the cache neither under-counts them nor frees them while in flight.
+static int stage_segment(Plan& P, int si) {
+  pb_segment_s* s = P.g->segs[si];
+  Context* ctx = P.ctx;
+  cudaStream_t cs = ctx->copy_stream;
+  std::lock_guard<std::mutex> lk(s->mu);
+  s->inflight++; P.r->pinned_segments = si + 1;
+  { std::lock_guard<std::mutex> lk2(ctx->mu); s->last_used = ++ctx->lru_clock; }
+  const int rc = stage_segment_columns(P, si);
   if (s->device_bytes != s->accounted_bytes) {
     std::lock_guard<std::mutex> lk2(ctx->mu);
     ctx->staged_bytes += s->device_bytes - s->accounted_bytes;
@@ -1838,6 +1872,9 @@ static int stage_segment(Plan& P, int si) {
     CU(cudaEventRecord(s->staged_ev, cs));
     s->stage_dirty = false; s->staged_pending = true;
   }
+  if (rc) return rc;
+  // the epochs the plan's pointers belong to, read while the segment is pinned (a replay compares them after pinning again)
+  P.r->rp.seg_epochs[(size_t)si] = s->epoch;
   if (s->staged_pending) {
     if (cudaEventQuery(s->staged_ev) == cudaSuccess) s->staged_pending = false;
     else { P.seg_wait[si] = s->staged_ev; P.n_pending++; }
@@ -1854,6 +1891,7 @@ static int stage_inputs(Plan& P) {
   P.acol.assign(n_segs, std::vector<int>(P.nA, -1));
   P.seg_wait.assign(n_segs, nullptr);
   P.seg_rg.assign(n_segs, nullptr);
+  P.r->rp.seg_epochs.assign(n_segs, 0);
   P.cand_leaf.resize(n_segs); P.cand_frac.resize(n_segs);
   for (int si = 0; si < n_segs; si++) plan_candidate_leaves(P.g->segs[si], P.sqs[si], P.cand_leaf[si], P.cand_frac[si]);
   for (int si = 0; si < n_segs; si++) if ((rc = stage_segment(P, si))) return rc;
@@ -2816,9 +2854,10 @@ static int exec_single(pb_segment_group_handle g, const pb_segment_query* sqs, c
   if (try_cache) {
     sig = plan_signature(g, sqs, q);
     if (pb_result_s* p = plan_take(g, sig)) {
-      if ((rc = replay_plan(p, q))) { free_result(p); return rc; }
-      *out = p;
-      return PB_OK;
+      rc = replay_plan(p, q);
+      if (rc == PB_OK) { *out = p; return PB_OK; }
+      if (rc != PB_REPLAY_STALE) { free_result(p); return rc; }
+      sig = plan_signature(g, sqs, q);               // (the retired plan's epochs are gone: key the new plan by the current ones)
     }
   }
   Plan P;
@@ -3653,6 +3692,7 @@ int pbi_plan_replay(pb_segment_group_handle g, const std::string& host_key, cons
   if (!p) return 0;
   DeviceGuard dg(g->ctx);
   int rc = replay_plan(p, q);
+  if (rc == PB_REPLAY_STALE) return 0;
   if (rc) { free_result(p); return rc; }
   *out = p;
   return 1;

@@ -53,10 +53,11 @@ def segment_sizes(rng, seed: int, max_total: int) -> List[int]:
     return sizes
 
 
-def make_tables(seed: int, max_total: int = 600_000) -> Tuple[list, List[Dict[str, Col]], dict]:
-    """(segments, per-segment source columns, facts about the table the tests use)"""
+def make_tables(seed: int, max_total: int = 600_000, sizes: List[int] = None) -> Tuple[list, List[Dict[str, Col]], dict]:
+    """(segments, per-segment source columns, facts about the table the tests use); sizes: the docs of each segment, in
+    place of the seed's choice"""
     rng = np.random.default_rng(77_000 + seed)
-    sizes = segment_sizes(rng, seed, max_total)
+    sizes = segment_sizes(rng, seed, max_total) if sizes is None else list(sizes)
     total = sum(sizes)
     # LONG metric: max|v| x docs of the whole call just inside or just outside 2^53 (plan_rows_kernel's exact-integer test)
     long_bound = int((2 ** 53) // total * (0.5 if seed % 2 == 0 else 2.0))
